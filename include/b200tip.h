@@ -25,6 +25,14 @@
  *   tip_kde_lse         scipy==1.4.1 gaussian_kernel_estimate pair loop (called from
  *                       src/core/stable_kde.py:101), in the log domain
  *   tip_kde_combine     merge of per-column-chunk (max, sum) partials
+ *   tip_kmeans_fit      src/core/surprise.py:117-118 KMeans(n_clusters=k, n_init, max_iter).fit (sklearn KMeans:
+ *                       greedy k-means++ seeding + Lloyd iterations, all n_init runs in one kernel)
+ *   tip_kmeans_predict  src/core/surprise.py:133 best_clusterer.predict (sklearn KMeans.predict), and the
+ *                       final relabel / inertia of a fit
+ *   tip_sil_prep        (new) operand packing of the silhouette pass
+ *   tip_sil_dsum        src/core/surprise.py:119 silhouette_score: the all-pairs Euclidean distance sums
+ *                       (sklearn pairwise_distances_chunked + np.bincount per cluster), as a wgmma pass
+ *   tip_sil_finish      sklearn silhouette_samples: a, b, (b - a) / max(a, b), nan -> 0
  */
 #ifndef B200TIP_H
 #define B200TIP_H
@@ -379,6 +387,50 @@ int tip_pair_prep_f16(const void* src, int dtype, int64_t rows, int64_t d, const
 /* merges `slots` partials per row in ascending slot order: out_max, out_sum (fp32) */
 int tip_kde_combine(const float* part_max, const float* part_sum, int64_t m, int32_t slots,
                     float* out_max, float* out_sum, void* stream);
+
+/* ---- k-means discriminator of MultiModalSA (surprise.py:102-133) ---------------------------------
+ * tip_kmeans_fit: x n x d (TIP_F32/TIP_F64, k <= n < 2^31), 1 <= k <= 64, 1 <= runs <= 64,
+ * runs * k * d < 2^31.  Runs `runs` independent fits (sklearn's n_init) in one persistent cooperative
+ * kernel.  Seeding: greedy k-means++ with 2 + int(ln k) trials per centre (first centre uniform,
+ * candidates drawn with probability ~ D^2, the candidate with the lowest potential is kept); draws
+ * come from a counter-based RNG keyed by (seed, k, run, step, trial).  Lloyd: nearest centre (squared
+ * Euclidean in the input dtype, ties: lowest index), centres = member means accumulated in double;
+ * an empty cluster takes the row farthest from its centre (sklearn _relocate_empty_clusters).  A run
+ * stops when no label changed, when sum ||centre shift||^2 <= tol (tol already scaled by the caller:
+ * mean(var(x, axis=0)) * tol), or after max_iter iterations.  Writes centers[runs x k x d] (input
+ * dtype) and n_iter[runs]; the final labels / inertia come from tip_kmeans_predict.  Deterministic:
+ * fixed-order reductions, no floating-point atomics.  work: tip_kmeans_work_bytes(...) bytes of
+ * scratch (-1: invalid arguments).  One call at a time per work buffer. */
+int64_t tip_kmeans_work_bytes(int64_t n, int64_t d, int32_t k, int32_t runs, int dtype);
+int tip_kmeans_fit(const void* x, int dtype, int64_t n, int64_t d, int32_t k, int32_t runs,
+                   int32_t max_iter, double tol, uint64_t seed, void* work, void* centers,
+                   int32_t* n_iter, void* stream);
+/* labels[r*n + i] = nearest of the k centres centers[r] (runs x k x d, input dtype) to row i (ties:
+ * lowest index); optional sqdist[r*n + i] (double) = its squared distance in the input dtype;
+ * optional inertia[r] = sum_i sqdist[r*n + i] (double, fixed order; needs sqdist). */
+int tip_kmeans_predict(const void* x, int dtype, int64_t n, int64_t d, const void* centers, int32_t k,
+                       int32_t runs, int32_t* labels, double* sqdist, double* inertia, void* stream);
+
+/* ---- silhouette score (sklearn.metrics.silhouette_samples) on the tensor cores ----------------------
+ * tip_sil_prep: the rows src_idx[r] (label-sorted order; NULL: r) of x, centred on `center`, packed as
+ * tip_pair_prep's three-segment operands — query role into q_pack, train role (scale -2, norm_coef 1)
+ * into t_pack, pitch tip_pair_pitch(d, 3) — except that the norm term is the one the operands carry,
+ * |h|^2 + 2<h, l>, so that identical rows give a distance of 0; sqnorm[rows] receives that norm.
+ * tip_sil_dsum: for every work item (a query tile x a span of columns inside ONE cluster) writes
+ * part_sum[slot*n + row] = sum over the span of sqrt(max(|x|^2 + |y|^2 - 2<x, y>, 0)), fp32, the row's
+ * own column excluded (queries and columns are the same sorted matrix).
+ * tip_sil_finish: out[out_idx[i]] (out_idx NULL: i) = silhouette value of sorted row i (double):
+ * per-cluster sums merged over the slots in ascending order (slot_cluster[slots], non-decreasing),
+ * a = sum_own / (n_own - 1), b = min over the other clusters of sum_c / n_c, (b - a) / max(a, b);
+ * 0 for singleton clusters and for a = b = 0.  labels_sorted[n], counts[clusters]. */
+int tip_sil_prep(const void* src, int dtype, int64_t rows, int64_t d, const float* center,
+                 const int32_t* src_idx, void* q_pack, void* t_pack, float* sqnorm, void* stream);
+int tip_sil_dsum(const void* q_pack, const void* t_pack, const float* sqnorm, int64_t n, int64_t d,
+                 int64_t pitch, const tip_work_item* items, int32_t n_items, float* part_sum,
+                 void* stream);
+int tip_sil_finish(const float* part_sum, int64_t n, int32_t slots, const int32_t* slot_cluster,
+                   const int32_t* labels_sorted, const int32_t* counts, const int32_t* out_idx,
+                   double* out, void* stream);
 
 /* ---- bring-up / validation: plain accumulator dump ------------------------------------
  * out[256*256] (fp32, row-major, leading dimension 256) = tail-augmented dot products of q rows

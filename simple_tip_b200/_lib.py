@@ -86,6 +86,13 @@ _SIGNATURES = {
     "tip_debug_timeline": (C.c_int, [_vp, _i32]),
     "tip_debug_cta_clock": (C.c_int, [_vp]),
     "tip_pair_probe": (C.c_int, [_vp, _i64, _vp, _i64, _i64, C.c_int, _i64, C.c_int, _vp, _vp]),
+    "tip_kmeans_work_bytes": (_i64, [_i64, _i64, _i32, _i32, C.c_int]),
+    "tip_kmeans_fit": (C.c_int, [_vp, C.c_int, _i64, _i64, _i32, _i32, _i32, C.c_double, C.c_uint64, _vp, _vp, _vp,
+                                 _vp]),
+    "tip_kmeans_predict": (C.c_int, [_vp, C.c_int, _i64, _i64, _vp, _i32, _i32, _vp, _vp, _vp, _vp]),
+    "tip_sil_prep": (C.c_int, [_vp, C.c_int, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "tip_sil_dsum": (C.c_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp, _i32, _vp, _vp]),
+    "tip_sil_finish": (C.c_int, [_vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
 }
 
 _lock = threading.Lock()

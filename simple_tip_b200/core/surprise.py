@@ -92,24 +92,58 @@ def _by_class_discriminator(activations: Activations, predictions: Predictions) 
     return _class_predictions(predictions)
 
 
+def _kmeans_backend(backend: Optional[str]) -> str:
+    """backend=None: the B200TIP_KMEANS environment variable, default "sklearn"."""
+    backend = backend if backend is not None else os.environ.get("B200TIP_KMEANS", "sklearn")
+    if backend not in ("sklearn", "device"):
+        raise ValueError(f"backend must be 'sklearn' or 'device', got {backend!r}")
+    return backend
+
+
+def _trace_matrix(activations):
+    """[N, D] traces: the device matrix for torch CUDA traces, else the reference's host flattening."""
+    from .. import engine as E
+
+    x = E.device_matrix(activations)
+    return x if x is not None else _flatten_layers(activations)
+
+
 class _KmeansDiscriminator:
-    """k-means modal assignment with silhouette model selection (surprise.py:102-133);
-    sklearn on the host — outside the accelerated path (SURVEY.md §2 row 3)."""
+    """k-means modal assignment with silhouette model selection (surprise.py:102-133).
+    backend="sklearn" (default): sklearn on the host, as the reference.  backend="device": k-means and the
+    silhouette score on the GPU (core/clustering.py), seeded with `random_state` (the reference's sklearn call
+    is unseeded); the traces may then be torch CUDA tensors."""
 
     def __init__(self, training_data: Activations, potential_k: Iterable[int], subsampling=1.0,
-                 subsampling_seed: int = 0, n_init: int = 10, max_iter: int = 300):
-        from sklearn.cluster import KMeans
-        from sklearn.metrics import silhouette_score
+                 subsampling_seed: int = 0, n_init: int = 10, max_iter: int = 300, backend: Optional[str] = None,
+                 random_state: int = 0):
+        self.backend = _kmeans_backend(backend)
+        if self.backend == "device":
+            from .. import engine as E
+            from .clustering import KMeans, silhouette_score
 
-        data = _subsample_array(subsampling, _flatten_layers(training_data), seed=subsampling_seed)
+            E.require_cuda()
+            data = _subsample_array(subsampling, _trace_matrix(training_data), seed=subsampling_seed)
+        else:
+            from sklearn.cluster import KMeans
+            from sklearn.metrics import silhouette_score
+
+            data = _subsample_array(subsampling, _flatten_layers(training_data), seed=subsampling_seed)
         self.best_score, self.best_k, self.best_clusterer = -np.inf, None, None
         for k in potential_k:
-            km = KMeans(n_clusters=k, n_init=n_init, max_iter=max_iter)
+            if self.backend == "device":
+                km = KMeans(n_clusters=k, n_init=n_init, max_iter=max_iter, random_state=random_state)
+            else:
+                km = KMeans(n_clusters=k, n_init=n_init, max_iter=max_iter)
             score = silhouette_score(data, km.fit_predict(data))
             if score > self.best_score:
                 self.best_score, self.best_k, self.best_clusterer = score, k, km
 
     def __call__(self, activations: Activations, predictions: Predictions) -> np.ndarray:
+        if self.backend == "device":
+            from .. import engine as E
+
+            return E.host_array(self.best_clusterer.predict(_trace_matrix(activations)))
         return self.best_clusterer.predict(_flatten_layers(activations))
 
 
@@ -170,9 +204,19 @@ class MultiModalSA(SA):
 
     @staticmethod
     def build_with_kmeans(activations, predictions, sa_constructor, potential_k: Iterable[int], n_init: int = 10,
-                          max_iter: int = 300, subsampling=1.0, subsampling_seed: int = 0) -> "MultiModalSA":
+                          max_iter: int = 300, subsampling=1.0, subsampling_seed: int = 0,
+                          backend: Optional[str] = None, random_state: int = 0) -> "MultiModalSA":
+        """backend / random_state: see _KmeansDiscriminator (B200TIP_KMEANS=device selects the GPU backend)."""
         disc = _KmeansDiscriminator(activations, potential_k, n_init=n_init, max_iter=max_iter,
-                                    subsampling=subsampling, subsampling_seed=subsampling_seed)
+                                    subsampling=subsampling, subsampling_seed=subsampling_seed, backend=backend,
+                                    random_state=random_state)
+        if disc.backend == "device":
+            # the modal SAs are fitted on host rows, as the reference does
+            from .. import engine as E
+
+            x = E.device_matrix(activations)
+            if x is not None:
+                activations = x.cpu().numpy()
         return MultiModalSA.build(activations, predictions, disc, sa_constructor)
 
     @staticmethod
@@ -194,7 +238,8 @@ class MultiModalSA(SA):
 
     def __call__(self, activations, predictions, num_threads: int = 1) -> np.ndarray:
         modal = self.discriminator(activations, predictions)
-        acts = _flatten_layers(activations)
+        on_device = isinstance(self.discriminator, _KmeansDiscriminator) and self.discriminator.backend == "device"
+        acts = _trace_matrix(activations) if on_device else _flatten_layers(activations)
         preds = _flatten_predictions(predictions)
         assert len(modal) == acts.shape[0], (
             f"The discriminator returned an invalid number ({len(modal)}) of modal indexes."
@@ -208,7 +253,8 @@ class MultiModalSA(SA):
         # result copy are launched before the first result is waited for (`score_begin` / `finish`).
         per_modal = None
         ours = all(isinstance(sa, (LSA, MDSA, MLSA, DSA)) for sa in sas)    # user-defined SAs keep getting NumPy arrays
-        if ours and isinstance(acts, np.ndarray) and acts.dtype in (np.float32, np.float64) and len(present) > 1:
+        float_rows = not isinstance(acts, np.ndarray) or acts.dtype in (np.float32, np.float64)   # device traces: checked later
+        if ours and float_rows and len(present) > 1:
             try:
                 import torch
 
@@ -232,7 +278,8 @@ class MultiModalSA(SA):
             per_modal = []
             for sa, mid in zip(sas, present):
                 rows = modal == mid
-                per_modal.append(sa(acts[rows], None if preds is None else preds[rows], num_threads=num_threads))
+                sel = acts[rows] if isinstance(acts, np.ndarray) else _take_rows(acts, np.flatnonzero(rows))
+                per_modal.append(sa(sel, None if preds is None else preds[rows], num_threads=num_threads))
         res = np.full(fill_value=-np.inf, shape=modal.shape, dtype=per_modal[0].dtype)
         for mid, vals in zip(present, per_modal):
             res[modal == mid] = vals

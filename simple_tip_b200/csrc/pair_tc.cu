@@ -8,6 +8,8 @@
 // tip_pair_prep) and reduces it on the fly — no N_test x N_train intermediate ever leaves the SM:
 //   MODE_NN   per-row running minimum + candidate emission (DSA, surprise.py:638-647)
 //   MODE_LSE  per-row online log-sum-exp (LSA / Gaussian KDE, scipy 1.4.1 gaussian_kernel_estimate)
+//   MODE_DSUM per-row sum of Euclidean distances over the item's span (silhouette score, sklearn
+//             silhouette_samples); the query's own column contributes 0
 //   MODE_DUMP raw accumulator tile (bring-up / validation)
 //
 // Roles (384 threads): warpgroup 0 = TMA producer and work-item hand-out (one lane); warpgroups 1
@@ -49,7 +51,7 @@ static_assert(kSmemBytes <= kSmemMax, "pair kernel does not fit");
 // tip_nn_filter keeps the query tile resident for packed rows of at most this many K16 steps (d <= 128)
 constexpr int kRsMaxK16 = 9;
 
-enum { MODE_NN = 0, MODE_LSE = 1, MODE_DUMP = 2 };
+enum { MODE_NN = 0, MODE_LSE = 1, MODE_DUMP = 2, MODE_DSUM = 3 };
 
 struct PairArgs {
   const tip_work_item* items;
@@ -71,7 +73,7 @@ struct PairArgs {
   int32_t* cand_idx;
   int32_t* cand_cnt;
   int cap;
-  // MODE_LSE
+  // MODE_LSE (MODE_DSUM: part_sum only)
   float* part_max;
   float* part_sum;
   // MODE_DUMP
@@ -180,6 +182,7 @@ struct EpiState {
   float nx, e2, g, best, thr, s_ref;   // MODE_NN (identical in the four lanes of the row's quad)
   int n_staged;                        // MODE_NN, kept by the quad's first lane only
   float run_max, run_sum;              // MODE_LSE
+  double dsum;                         // MODE_DSUM
 };
 struct EpiShared {
   float* cand_val;
@@ -291,6 +294,26 @@ __device__ __forceinline__ void epi_chunk(const PairArgs& args, EpiState& st, co
     s += __shfl_xor_sync(0xffffffffu, s, 1);     // IEEE addition is commutative: the four lanes agree
     s += __shfl_xor_sync(0xffffffffu, s, 2);
     st.run_sum += s;
+  } else if (MODE == MODE_DSUM) {
+    // acc = |y|^2 - 2<x, y>: + |x|^2, clamp, sqrt.  Columns past the span and the query's own column add 0.
+    float dd[8];
+#pragma unroll
+    for (int k = 0; k < 8; k++) {
+      float r;
+      asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(fmaxf(v[k] + st.nx, 0.f)));
+      dd[k] = r;
+    }
+    if (partial || (EXCL && cbase < st.ex_hi && cbase + 32 > st.ex_lo)) {
+#pragma unroll
+      for (int k = 0; k < 8; k++) {
+        const int c = cbase + 8 * (k >> 1) + 2 * sub + (k & 1);
+        if (c >= st.col1 || (EXCL && c >= st.ex_lo && c < st.ex_hi)) dd[k] = 0.f;
+      }
+    }
+    float s = ((dd[0] + dd[4]) + (dd[1] + dd[5])) + ((dd[2] + dd[6]) + (dd[3] + dd[7]));
+    s += __shfl_xor_sync(0xffffffffu, s, 1);
+    s += __shfl_xor_sync(0xffffffffu, s, 2);
+    st.dsum += (double)s;
   }
 }
 
@@ -430,9 +453,13 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         s.valid_row = row_local < it.q_rows;
         s.row = (int64_t)it.q_row0 + row_local;
         s.nx = 0.f; s.e2 = 0.f; s.g = 0.f; s.best = kInf; s.thr = kInf; s.s_ref = kInf; s.n_staged = 0;
-        s.run_max = -kInf; s.run_sum = 0.f;
+        s.run_max = -kInf; s.run_sum = 0.f; s.dsum = 0.0;
         s.col1 = it.col1;
         s.ex_lo = 0; s.ex_hi = 0;
+        if (MODE == MODE_DSUM && s.valid_row) {
+          s.nx = args.q_sqnorm[s.row];
+          if (EXCL) { s.ex_lo = (int)s.row; s.ex_hi = (int)s.row + 1; }   // queries and columns: one matrix
+        }
         uint32_t ref_bits = 0x7f800000u;
         if (MODE == MODE_NN && s.valid_row) {
           if (EXCL && (it.reserved & 1) && args.q_class) {
@@ -558,6 +585,8 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         } else if (MODE == MODE_LSE) {
           args.part_max[(int64_t)it.slot * args.m + s.row] = s.run_max;
           args.part_sum[(int64_t)it.slot * args.m + s.row] = s.run_sum;
+        } else if (MODE == MODE_DSUM) {
+          args.part_sum[(int64_t)it.slot * args.m + s.row] = (float)s.dsum;
         }
       }
       __syncwarp();
@@ -742,6 +771,18 @@ extern "C" int tip_kde_lse_f16(const void* q_pack, int64_t m, const void* t_pack
   a.part_max = part_max; a.part_sum = part_sum;
   const bool resa = (a.k16 + 3) / 4 <= kResAChunks;
   return launch_pair<MODE_LSE, false, true>(q_pack, m, t_pack, n, pitch, a, resa, (cudaStream_t)stream);
+}
+
+extern "C" int tip_sil_dsum(const void* q_pack, const void* t_pack, const float* sqnorm, int64_t n, int64_t d,
+                            int64_t pitch, const tip_work_item* items, int32_t n_items, float* part_sum, void* stream) {
+  TIP_REQUIRE(q_pack && t_pack && sqnorm && items && part_sum, "null pointer");
+  TIP_REQUIRE(pitch == tip_pair_pitch(d, 3), "pitch does not match tip_pair_pitch(d, 3)");
+  if (n_items == 0) return TIP_OK;
+  PairArgs a{};
+  a.items = items; a.n_items = n_items; a.n_static = n_items; a.k16 = k16_of(d, 3); a.m = n;
+  a.q_sqnorm = sqnorm; a.part_sum = part_sum;
+  const bool resa = (a.k16 + 3) / 4 <= kResAChunks;
+  return launch_pair<MODE_DSUM, true>(q_pack, n, t_pack, n, pitch, a, resa, (cudaStream_t)stream);
 }
 
 extern "C" int tip_pair_probe(const void* q_pack, int64_t m, const void* t_pack, int64_t n, int64_t d, int segments,

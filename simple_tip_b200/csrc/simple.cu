@@ -541,7 +541,7 @@ __global__ void __launch_bounds__(256) pair_prep_kernel(const T* __restrict__ sr
                                                         __nv_bfloat16* __restrict__ dst, int64_t pitch,
                                                         float* __restrict__ sqnorm, float* __restrict__ rounderr,
                                                         uint32_t* __restrict__ row_min, int32_t* __restrict__ cand_cnt,
-                                                        const int32_t* __restrict__ src_idx) {
+                                                        const int32_t* __restrict__ src_idx, bool trunc_norm) {
   const int lane = threadIdx.x & 31;
   const int64_t row = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
   if (row >= rows) return;
@@ -566,7 +566,10 @@ __global__ void __launch_bounds__(256) pair_prep_kernel(const T* __restrict__ sr
       const __nv_bfloat16 l = __float2bfloat16_rn(__fsub_rn(v, hf));
       const float res = __fsub_rn(__fsub_rn(v, hf), __bfloat162float(l));
       err += (double)res * (double)res;
-      acc += (double)v * (double)v;
+      // trunc_norm: the norm the operands themselves carry, |h|^2 + 2<h, l> (the K-loop never forms l*l), so
+      // that |x|^2 + |y|^2 - 2<x, y> cancels for identical rows
+      const double hd = hf, ld = __bfloat162float(l);
+      acc += trunc_norm ? hd * hd + 2.0 * hd * ld : (double)v * (double)v;
       if (role == TIP_ROLE_TRAIN) {
         const __nv_bfloat16 sh = __float2bfloat16_rn(scale * hf);
         out[c] = sh;
@@ -907,7 +910,8 @@ extern "C" int64_t tip_pair_pitch(int64_t d, int segments) {
 
 static int pair_prep_impl(const void* src, int dtype, int64_t rows, int64_t d, const float* center, int role,
                           int segments, float scale, float norm_coef, void* dst, float* sqnorm, float* rounderr,
-                          uint32_t* row_min, int32_t* cand_cnt, const int32_t* src_idx, void* stream) {
+                          uint32_t* row_min, int32_t* cand_cnt, const int32_t* src_idx, void* stream,
+                          bool trunc_norm = false) {
   TIP_REQUIRE(src && dst, "null pointer");
   TIP_REQUIRE(segments == 1 || segments == 3, "segments must be 1 or 3");
   TIP_REQUIRE(role == TIP_ROLE_QUERY || role == TIP_ROLE_TRAIN, "role");
@@ -923,11 +927,11 @@ static int pair_prep_impl(const void* src, int dtype, int64_t rows, int64_t d, c
   if (dtype == TIP_F32)
     pair_prep_kernel<float><<<(unsigned)blocks, 256, 0, st>>>((const float*)src, rows, (int)d, center, role, segments,
                                                              scale, norm_coef, (__nv_bfloat16*)dst, pitch, sqnorm,
-                                                             rounderr, row_min, cand_cnt, src_idx);
+                                                             rounderr, row_min, cand_cnt, src_idx, trunc_norm);
   else if (dtype == TIP_F64)
     pair_prep_kernel<double><<<(unsigned)blocks, 256, 0, st>>>((const double*)src, rows, (int)d, center, role,
                                                               segments, scale, norm_coef, (__nv_bfloat16*)dst, pitch,
-                                                              sqnorm, rounderr, row_min, cand_cnt, src_idx);
+                                                              sqnorm, rounderr, row_min, cand_cnt, src_idx, trunc_norm);
   else
     TIP_REQUIRE(false, "dtype must be TIP_F32 or TIP_F64");
   TIP_LAUNCH_CHECK();
@@ -939,6 +943,16 @@ extern "C" int tip_pair_prep(const void* src, int dtype, int64_t rows, int64_t d
                              void* stream) {
   return pair_prep_impl(src, dtype, rows, d, center, role, segments, scale, norm_coef, dst, sqnorm, rounderr, nullptr,
                         nullptr, nullptr, stream);
+}
+
+extern "C" int tip_sil_prep(const void* src, int dtype, int64_t rows, int64_t d, const float* center,
+                            const int32_t* src_idx, void* q_pack, void* t_pack, float* sqnorm, void* stream) {
+  TIP_REQUIRE(q_pack && t_pack && sqnorm, "null pointer");
+  const int rc = pair_prep_impl(src, dtype, rows, d, center, TIP_ROLE_QUERY, 3, 1.f, 0.f, q_pack, sqnorm, nullptr,
+                                nullptr, nullptr, src_idx, stream, true);
+  if (rc != TIP_OK) return rc;
+  return pair_prep_impl(src, dtype, rows, d, center, TIP_ROLE_TRAIN, 3, -2.f, 1.f, t_pack, nullptr, nullptr, nullptr,
+                        nullptr, src_idx, stream, true);
 }
 
 extern "C" int tip_pair_prep_f16(const void* src, int dtype, int64_t rows, int64_t d, const float* center, int role,

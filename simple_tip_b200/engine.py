@@ -1247,3 +1247,107 @@ def quadratic_forms(x, centres: Sequence[Tuple[torch.Tensor, torch.Tensor]], col
         if m:
             _lib.check(lib.tip_row_sqnorm(_p(y), m, y.shape[1], _p(out[k]), _stream()), "tip_row_sqnorm")
     return out
+
+
+# ------------------------------------------------------------------------------------------
+# k-means discriminator of MultiModalSA (surprise.py:102-133): device k-means + silhouette
+# ------------------------------------------------------------------------------------------
+KMEANS_MAX_K = 64
+
+
+def silhouette_items(counts: np.ndarray, span_tiles: int, row_tile: int = _lib.ROW_TILE,
+                     col_tile: int = _lib.COL_TILE) -> Tuple[np.ndarray, np.ndarray]:
+    """Work list of the silhouette pass over label-sorted rows (cluster c = rows [off[c], off[c+1])): every
+    query tile x every span of columns inside ONE cluster, so that each partial-sum slot belongs to one
+    cluster.  Returns (items [n, 6] in span-major order, slot_cluster [slots] int32, non-decreasing)."""
+    counts = np.asarray(counts, dtype=np.int64)
+    off = np.zeros(len(counts) + 1, dtype=np.int64)
+    np.cumsum(counts, out=off[1:])
+    n = int(off[-1])
+    ranges = [[(int(off[c]), int(off[c + 1])) for c in range(len(counts)) if counts[c] > 0]]
+    items, _ = build_items(np.array([0, n], dtype=np.int64), ranges, span_tiles, row_tile, col_tile)
+    slots = int(items[:, 4].max()) + 1 if items.shape[0] else 0
+    slot_cluster = np.zeros(slots, dtype=np.int32)
+    slot_cluster[items[:, 4]] = np.searchsorted(off, items[:, 2], side="right") - 1
+    return span_major(items), slot_cluster
+
+
+def _device_sms(lib) -> int:
+    sms = C.c_int(0)
+    _lib.check(lib.tip_device_info(C.byref(sms), None, None), "tip_device_info")
+    return sms.value
+
+
+def kmeans_fit(x: torch.Tensor, k: int, n_init: int, max_iter: int, tol: float, seed: int):
+    """All n_init runs of sklearn's KMeans(k, init="k-means++", algorithm="lloyd") on the [n, d] device matrix x
+    (float32 / float64): one cooperative kernel for seeding + Lloyd, one predict launch for the final labels and
+    inertia of every run.  Returns (centres [k, d] x.dtype, labels [n] int32, inertia, n_iter) of the run with
+    the lowest inertia (ties: the lowest run), all but the two scalars on the device."""
+    lib = _lib.load()
+    n, d = x.shape
+    dt = tip_dtype(x.dtype)
+    tol_abs = float(torch.var(x, dim=0, correction=0).mean()) * tol if tol > 0 else 0.0
+    wb = int(lib.tip_kmeans_work_bytes(n, d, k, n_init, dt))
+    if wb < 0:
+        raise ValueError(f"k-means of {n} x {d} rows with k={k}, n_init={n_init} is not supported: "
+                         f"{lib.tip_last_error().decode(errors='replace')}")
+    work = torch.empty(wb, dtype=torch.uint8, device=x.device)
+    cen = torch.empty((n_init, k, d), dtype=x.dtype, device=x.device)
+    n_iter = torch.zeros(n_init, dtype=torch.int32, device=x.device)
+    _lib.check(lib.tip_kmeans_fit(_p(x), dt, n, d, k, n_init, max_iter, tol_abs, seed & (2 ** 64 - 1), _p(work),
+                                  _p(cen), _p(n_iter), _stream()), "tip_kmeans_fit")
+    del work
+    labels = torch.empty((n_init, n), dtype=torch.int32, device=x.device)
+    sq = torch.empty((n_init, n), dtype=torch.float64, device=x.device)
+    inertia = torch.empty(n_init, dtype=torch.float64, device=x.device)
+    _lib.check(lib.tip_kmeans_predict(_p(x), dt, n, d, _p(cen), k, n_init, _p(labels), _p(sq), _p(inertia), _stream()),
+               "tip_kmeans_predict")
+    inert = inertia.cpu().numpy()
+    best = int(np.argmin(inert))          # first minimum: ties go to the lowest run
+    return cen[best].clone(), labels[best].clone(), float(inert[best]), int(n_iter[best].item())
+
+
+def kmeans_predict(x: torch.Tensor, centres: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Nearest centre of every row (ties: lowest index) and its squared distance (float64), on the device."""
+    lib = _lib.load()
+    n, d = x.shape
+    centres = centres.to(device=x.device, dtype=x.dtype).contiguous()
+    labels = torch.empty(n, dtype=torch.int32, device=x.device)
+    sq = torch.empty(n, dtype=torch.float64, device=x.device)
+    _lib.check(lib.tip_kmeans_predict(_p(x), tip_dtype(x.dtype), n, d, _p(centres), centres.shape[0], 1, _p(labels),
+                                      _p(sq), None, _stream()), "tip_kmeans_predict")
+    return labels, sq
+
+
+def silhouette_samples(x: torch.Tensor, labels: torch.Tensor, n_clusters: int) -> torch.Tensor:
+    """sklearn silhouette_samples of the [n, d] device matrix x (float32 / float64) under labels in
+    [0, n_clusters) (every cluster non-empty): label-sorted, packed once in both roles, one wgmma pass of
+    per-(row, cluster span) distance sums, one finishing kernel.  Returns float64 [n] in x's row order."""
+    lib = _lib.load()
+    n, d = x.shape
+    lab = labels.to(torch.int64)
+    order = torch.argsort(lab, stable=True)
+    counts = torch.bincount(lab, minlength=n_clusters)
+    counts_h = counts.cpu().numpy()
+    order32 = order.to(torch.int32)
+    lab_sorted = lab.index_select(0, order).to(torch.int32)
+    counts32 = counts.to(torch.int32)
+    center = x.mean(dim=0).to(torch.float32)
+    pitch = int(lib.tip_pair_pitch(d, 3))
+    q_pack = torch.empty((n, pitch), dtype=torch.bfloat16, device=x.device)
+    t_pack = torch.empty((n, pitch), dtype=torch.bfloat16, device=x.device)
+    sq = torch.empty(n, dtype=torch.float32, device=x.device)
+    _lib.check(lib.tip_sil_prep(_p(x), tip_dtype(x.dtype), n, d, _p(center), _p(order32), _p(q_pack), _p(t_pack),
+                                _p(sq), _stream()), "tip_sil_prep")
+    pairs = math.ceil(n / _lib.ROW_TILE) * math.ceil(n / _lib.COL_TILE)
+    items, slot_cluster = silhouette_items(counts_h, span_tiles_for(pairs, _device_sms(lib)))
+    slots = slot_cluster.shape[0]
+    items_dev = torch.from_numpy(items).to(x.device)
+    slot_dev = torch.from_numpy(slot_cluster).to(x.device)
+    part = torch.zeros((slots, n), dtype=torch.float32, device=x.device)
+    _lib.check(lib.tip_sil_dsum(_p(q_pack), _p(t_pack), _p(sq), n, d, pitch, _p(items_dev), items.shape[0], _p(part),
+                                _stream()), "tip_sil_dsum")
+    out = torch.empty(n, dtype=torch.float64, device=x.device)
+    _lib.check(lib.tip_sil_finish(_p(part), n, slots, _p(slot_dev), _p(lab_sorted), _p(counts32), _p(order32), _p(out),
+                                  _stream()), "tip_sil_finish")
+    return out
