@@ -390,15 +390,20 @@ int tip_kde_combine(const float* part_max, const float* part_sum, int64_t m, int
 
 /* ---- k-means discriminator of MultiModalSA (surprise.py:102-133) ---------------------------------
  * tip_kmeans_fit: x n x d (TIP_F32/TIP_F64, k <= n < 2^31), 1 <= k <= 64, 1 <= runs <= 64,
- * runs * k * d < 2^31.  Runs `runs` independent fits (sklearn's n_init) in one persistent cooperative
+ * runs * k * d < 2^31, max_iter >= 0, tol >= 0.  Runs `runs` independent fits (sklearn's n_init) in one persistent cooperative
  * kernel.  Seeding: greedy k-means++ with 2 + int(ln k) trials per centre (first centre uniform,
  * candidates drawn with probability ~ D^2, the candidate with the lowest potential is kept); draws
  * come from a counter-based RNG keyed by (seed, k, run, step, trial).  Lloyd: nearest centre (squared
- * Euclidean in the input dtype, ties: lowest index), centres = member means accumulated in double;
- * an empty cluster takes the row farthest from its centre (sklearn _relocate_empty_clusters).  A run
- * stops when no label changed, when sum ||centre shift||^2 <= tol (tol already scaled by the caller:
- * mean(var(x, axis=0)) * tol), or after max_iter iterations.  Writes centers[runs x k x d] (input
- * dtype) and n_iter[runs]; the final labels / inertia come from tip_kmeans_predict.  Deterministic:
+ * Euclidean in the input dtype, ties: lowest index), centres = member means accumulated in double.
+ * Empty clusters (sklearn _relocate_empty_clusters): the set of empty clusters is fixed before any
+ * row moves; in ascending cluster order each takes the row farthest from its centre (descending
+ * distance, ties: lowest row), so a donor emptied by a move stays empty until the next assignment;
+ * nothing moves when every row sits exactly on its centre (more clusters than distinct rows); a
+ * cluster still empty keeps its previous centre.  A run stops when no label changed, when
+ * sum ||centre shift||^2 <= tol (tol already scaled by the caller: mean(var(x, axis=0)) * tol), or
+ * after max_iter iterations.  max_iter = 0 runs the seeding alone (centers = the seeds, n_iter = 0).
+ * Writes centers[runs x k x d] (input dtype) and n_iter[runs]; the final labels / inertia come from
+ * tip_kmeans_predict.  Deterministic:
  * fixed-order reductions, no floating-point atomics.  work: tip_kmeans_work_bytes(...) bytes of
  * scratch (-1: invalid arguments).  One call at a time per work buffer. */
 int64_t tip_kmeans_work_bytes(int64_t n, int64_t d, int32_t k, int32_t runs, int dtype);

@@ -125,6 +125,7 @@ __global__ void __launch_bounds__(kKmThreads, 1) kmeans_fit_kernel(const KmArgs 
   __shared__ int s_best[64];
   __shared__ int s_changed[64];
   __shared__ int64_t s_taken[kKmMaxK];
+  __shared__ int s_empty[kKmMaxK];
 
   const T* X = (const T*)a.x;
   T* C = (T*)a.cen;
@@ -295,15 +296,28 @@ __global__ void __launch_bounds__(kKmThreads, 1) kmeans_fit_kernel(const KmArgs 
       ch = __syncthreads_or(ch);
       int32_t* cnt = a.cnt + (int64_t)r * K;
       double* sums = a.sums + (int64_t)r * K * D;
-      int n_taken = 0;
+      // sklearn _relocate_empty_clusters: the set of empty clusters is fixed before any row moves (a donor emptied
+      // here stays empty until the next assignment), and nothing moves when every row sits on its centre
+      int n_empty = 0;
       for (int c = 0; c < K; c++) {
         if (cnt[c] != 0) continue;   // block-uniform (written before the last grid.sync)
-        // sklearn _relocate_empty_clusters: the row farthest from its centre moves to the empty cluster
+        if (tid == 0) s_empty[n_empty] = c;
+        n_empty++;
+      }
+      __syncthreads();
+      if (n_empty > 0) {
+        double mx = 0.0;
+        for (int64_t i = tid; i < n; i += kKmThreads) mx = fmax(mx, a.dist[(int64_t)r * n + i]);
+        if (!__syncthreads_or(mx > 0.0)) n_empty = 0;
+      }
+      for (int q = 0; q < n_empty; q++) {
+        const int c = s_empty[q];
+        // the row farthest from its centre (descending over the empty clusters, ties: lowest row) moves to c
         double bv = -1.0;
         int64_t bi = n;
         for (int64_t i = tid; i < n; i += kKmThreads) {
           bool taken = false;
-          for (int q = 0; q < n_taken; q++) taken |= s_taken[q] == i;
+          for (int j = 0; j < q; j++) taken |= s_taken[j] == i;
           const double v = a.dist[(int64_t)r * n + i];
           if (!taken && v > bv) { bv = v; bi = i; }
         }
@@ -315,8 +329,7 @@ __global__ void __launch_bounds__(kKmThreads, 1) kmeans_fit_kernel(const KmArgs 
           sums[(int64_t)c * D + j] = xv;
         }
         __syncthreads();
-        if (tid == 0) { cnt[donor] -= 1; cnt[c] = 1; s_taken[n_taken] = far; }
-        n_taken++;
+        if (tid == 0) { cnt[donor] -= 1; cnt[c] = 1; s_taken[q] = far; }
         __syncthreads();
       }
       double shift = 0.0;
@@ -476,7 +489,7 @@ extern "C" int tip_kmeans_fit(const void* x, int dtype, int64_t n, int64_t d, in
   int rc = km_check(dtype, n, d, k, runs);
   if (rc != TIP_OK) return rc;
   TIP_REQUIRE(x && work && centers && n_iter, "null pointer");
-  TIP_REQUIRE(max_iter >= 1 && tol >= 0.0, "max_iter / tol");
+  TIP_REQUIRE(max_iter >= 0 && tol >= 0.0, "max_iter / tol");   // max_iter 0: the k-means++ seeds alone
   int grid = 0;
   rc = dtype == TIP_F32 ? km_grid<float>(n, (int)d, k, runs, &grid) : km_grid<double>(n, (int)d, k, runs, &grid);
   if (rc != TIP_OK) return rc;

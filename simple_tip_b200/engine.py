@@ -1282,7 +1282,10 @@ def kmeans_fit(x: torch.Tensor, k: int, n_init: int, max_iter: int, tol: float, 
     """All n_init runs of sklearn's KMeans(k, init="k-means++", algorithm="lloyd") on the [n, d] device matrix x
     (float32 / float64): one cooperative kernel for seeding + Lloyd, one predict launch for the final labels and
     inertia of every run.  Returns (centres [k, d] x.dtype, labels [n] int32, inertia, n_iter) of the run with
-    the lowest inertia (ties: the lowest run), all but the two scalars on the device."""
+    the lowest inertia (ties: the lowest run), all but the two scalars on the device.  max_iter = 0 stops after
+    the seeding: the centres are the k-means++ seeds and n_iter is 0."""
+    if max_iter < 0 or tol < 0:
+        raise ValueError("max_iter must be >= 0 and tol >= 0")
     lib = _lib.load()
     n, d = x.shape
     dt = tip_dtype(x.dtype)
