@@ -1322,10 +1322,13 @@ def kmeans_predict(x: torch.Tensor, centres: torch.Tensor) -> Tuple[torch.Tensor
     return labels, sq
 
 
-def silhouette_samples(x: torch.Tensor, labels: torch.Tensor, n_clusters: int) -> torch.Tensor:
+def silhouette_samples(x: torch.Tensor, labels: torch.Tensor, n_clusters: int,
+                       span_tiles: Optional[int] = None) -> torch.Tensor:
     """sklearn silhouette_samples of the [n, d] device matrix x (float32 / float64) under labels in
     [0, n_clusters) (every cluster non-empty): label-sorted, packed once in both roles, one wgmma pass of
-    per-(row, cluster span) distance sums, one finishing kernel.  Returns float64 [n] in x's row order."""
+    per-(row, cluster span) distance sums, one finishing kernel.  Returns float64 [n] in x's row order.
+    span_tiles: column tiles per work-item span (None: span_tiles_for's choice for this card), so that a test can
+    run the 1- and 16-tile layouts on any card."""
     lib = _lib.load()
     n, d = x.shape
     lab = labels.to(torch.int64)
@@ -1342,8 +1345,10 @@ def silhouette_samples(x: torch.Tensor, labels: torch.Tensor, n_clusters: int) -
     sq = torch.empty(n, dtype=torch.float32, device=x.device)
     _lib.check(lib.tip_sil_prep(_p(x), tip_dtype(x.dtype), n, d, _p(center), _p(order32), _p(q_pack), _p(t_pack),
                                 _p(sq), _stream()), "tip_sil_prep")
-    pairs = math.ceil(n / _lib.ROW_TILE) * math.ceil(n / _lib.COL_TILE)
-    items, slot_cluster = silhouette_items(counts_h, span_tiles_for(pairs, _device_sms(lib)))
+    if span_tiles is None:
+        pairs = math.ceil(n / _lib.ROW_TILE) * math.ceil(n / _lib.COL_TILE)
+        span_tiles = span_tiles_for(pairs, _device_sms(lib))
+    items, slot_cluster = silhouette_items(counts_h, span_tiles)
     slots = slot_cluster.shape[0]
     items_dev = torch.from_numpy(items).to(x.device)
     slot_dev = torch.from_numpy(slot_cluster).to(x.device)
