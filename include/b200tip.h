@@ -33,6 +33,11 @@
  *   tip_sil_dsum        src/core/surprise.py:119 silhouette_score: the all-pairs Euclidean distance sums
  *                       (sklearn pairwise_distances_chunked + np.bincount per cluster), as a wgmma pass
  *   tip_sil_finish      sklearn silhouette_samples: a, b, (b - a) / max(a, b), nan -> 0
+ *   tip_gmm_quad        src/core/surprise.py:508-509,518 GaussianMixture.fit / score_samples (sklearn
+ *                       _estimate_log_gaussian_prob, 'full': |X @ prec_chol - mu @ prec_chol|^2), fp64 DMMA
+ *   tip_gmm_resp        sklearn _estimate_log_prob_resp (logsumexp, exp(log_resp)) and _e_step's mean
+ *   tip_gmm_moments     sklearn _estimate_gaussian_parameters: nk = sum(resp) + 10 eps, means = resp.T @ X / nk
+ *   tip_gmm_scatter     sklearn _estimate_gaussian_covariances_full: (resp_k * diff.T) @ diff / nk + reg_covar I
  */
 #ifndef B200TIP_H
 #define B200TIP_H
@@ -436,6 +441,35 @@ int tip_sil_dsum(const void* q_pack, const void* t_pack, const float* sqnorm, in
 int tip_sil_finish(const float* part_sum, int64_t n, int32_t slots, const int32_t* slot_cluster,
                    const int32_t* labels_sorted, const int32_t* counts, const int32_t* out_idx,
                    double* out, void* stream);
+
+/* ---- Gaussian mixture EM (sklearn GaussianMixture, covariance_type="full"), float64 ------------------
+ * x n x d (TIP_F32/TIP_F64, widened exactly to double on load), 1 <= n < 2^31, 1 <= d <= 65536,
+ * 1 <= k <= 64.  Parameters are double: means[k x d], prec_chol[k x d x d] (upper triangular, sklearn's
+ * precisions_cholesky_; entries below the diagonal are never read), q / resp [k x n] (component-major).
+ * Deterministic: fixed-order reductions, no floating-point atomics; the work split depends on the shape only.
+ * tip_gmm_quad: q[j*n + i] = |(x_i - means_j) . prec_chol_j|^2 (centred first), fp64 tensor cores.
+ * tip_gmm_resp: per row a_j = (-(d log 2pi + q_j) / 2 + log_det[j]) + log_weights[j]; optional
+ *   lse[i] = logsumexp_j a_j (scipy order), labels[i] = first argmax_j a_j, resp[j*n + i] = exp(a_j - lse);
+ *   optional lower_bound (device double) = mean of lse, merged in a fixed order (needs work).
+ * tip_gmm_moments: nk[k] = sum_i resp + 10 eps(double), sums[k x d] = resp^T x, means = sums / nk; any
+ *   of the three outputs may be NULL.
+ * tip_gmm_scatter: S_j = sum_i resp[j*n+i] (x_i - means_j)(x_i - means_j)^T over lower-triangle tiles,
+ *   mirrored; out[k x d x d] = S (nk NULL) or S / nk[j] + reg_covar on the diagonal.  The rows are split
+ *   into tip_gmm_scatter_chunks(n, d, k, scatter_chunks) chunks (scatter_chunks 0: automatic; the count
+ *   shrinks until the partials fit 256 MB) merged in ascending order.
+ * work: tip_gmm_work_bytes(n, d, k, scatter_chunks) bytes, for any of the calls (-1: invalid). */
+int32_t tip_gmm_scatter_chunks(int64_t n, int64_t d, int32_t k, int32_t scatter_chunks);
+int64_t tip_gmm_work_bytes(int64_t n, int64_t d, int32_t k, int32_t scatter_chunks);
+int tip_gmm_quad(const void* x, int dtype, int64_t n, int64_t d, const double* means,
+                 const double* prec_chol, int32_t k, double* q, void* stream);
+int tip_gmm_resp(const double* q, int64_t n, int64_t d, int32_t k, const double* log_weights,
+                 const double* log_det, double* resp, double* lse, int64_t* labels, double* lower_bound,
+                 void* work, void* stream);
+int tip_gmm_moments(const void* x, int dtype, int64_t n, int64_t d, const double* resp, int32_t k,
+                    double* nk, double* sums, double* means, void* work, void* stream);
+int tip_gmm_scatter(const void* x, int dtype, int64_t n, int64_t d, const double* resp,
+                    const double* means, int32_t k, const double* nk, double reg_covar,
+                    int32_t scatter_chunks, double* out, void* work, void* stream);
 
 /* ---- bring-up / validation: plain accumulator dump ------------------------------------
  * out[256*256] (fp32, row-major, leading dimension 256) = tail-augmented dot products of q rows

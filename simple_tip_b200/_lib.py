@@ -93,6 +93,12 @@ _SIGNATURES = {
     "tip_sil_prep": (C.c_int, [_vp, C.c_int, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp]),
     "tip_sil_dsum": (C.c_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp, _i32, _vp, _vp]),
     "tip_sil_finish": (C.c_int, [_vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "tip_gmm_scatter_chunks": (_i32, [_i64, _i64, _i32, _i32]),
+    "tip_gmm_work_bytes": (_i64, [_i64, _i64, _i32, _i32]),
+    "tip_gmm_quad": (C.c_int, [_vp, C.c_int, _i64, _i64, _vp, _vp, _i32, _vp, _vp]),
+    "tip_gmm_resp": (C.c_int, [_vp, _i64, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "tip_gmm_moments": (C.c_int, [_vp, C.c_int, _i64, _i64, _vp, _i32, _vp, _vp, _vp, _vp, _vp]),
+    "tip_gmm_scatter": (C.c_int, [_vp, C.c_int, _i64, _i64, _vp, _vp, _i32, _vp, C.c_double, _i32, _vp, _vp, _vp]),
 }
 
 _lock = threading.Lock()

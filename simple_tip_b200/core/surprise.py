@@ -100,6 +100,14 @@ def _kmeans_backend(backend: Optional[str]) -> str:
     return backend
 
 
+def _gmm_backend(backend: Optional[str]) -> str:
+    """backend=None: the B200TIP_GMM environment variable, default "sklearn"."""
+    backend = backend if backend is not None else os.environ.get("B200TIP_GMM", "sklearn")
+    if backend not in ("sklearn", "device"):
+        raise ValueError(f"backend must be 'sklearn' or 'device', got {backend!r}")
+    return backend
+
+
 def _trace_matrix(activations):
     """[N, D] traces: the device matrix for torch CUDA traces, else the reference's host flattening."""
     from .. import engine as E
@@ -357,17 +365,29 @@ class MLSA(SA):
     mixture.  Fit = sklearn's `GaussianMixture` on the host as in the reference; score: per component
     y = (x - mu_k) . precisions_cholesky_k on the GPU (sklearn `_estimate_log_gaussian_prob`), squared row norms,
     then `-logsumexp_k(log w_k - (D log 2pi + |y|^2) / 2 + log det chol_k)` in float64 on the host — the tail of
-    `GaussianMixture.score_samples`."""
+    `GaussianMixture.score_samples`.
+    backend="sklearn" (default, or B200TIP_GMM unset): the fit is sklearn's on the host.  backend="device": the fit
+    runs on the GPU in float64 (core/mixture.py), its k-means start seeded with `random_state` (the reference's
+    sklearn call is unseeded); CUDA traces then stay on the device.  Scoring is the same for both."""
 
-    def __init__(self, activations: Activations, num_components: int = 2):
+    def __init__(self, activations: Activations, num_components: int = 2, *, backend: Optional[str] = None,
+                 random_state: int = 0):
         super().__init__()
-        from sklearn.mixture import GaussianMixture
-
         from .. import engine as E
 
-        host = E.device_matrix(activations)
-        acts = host.cpu().numpy() if host is not None else _flatten_layers(activations)
-        self.gmm = GaussianMixture(n_components=num_components)
+        self.backend = _gmm_backend(backend)
+        if self.backend == "device":
+            from .mixture import GaussianMixture
+
+            E.require_cuda()
+            acts = _trace_matrix(activations)
+            self.gmm = GaussianMixture(n_components=num_components, random_state=random_state)
+        else:
+            from sklearn.mixture import GaussianMixture
+
+            host = E.device_matrix(activations)
+            acts = host.cpu().numpy() if host is not None else _flatten_layers(activations)
+            self.gmm = GaussianMixture(n_components=num_components)
         self.gmm.fit(acts)
         self._width = int(acts.shape[1])
         self._centres = None

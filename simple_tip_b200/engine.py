@@ -1322,6 +1322,197 @@ def kmeans_predict(x: torch.Tensor, centres: torch.Tensor) -> Tuple[torch.Tensor
     return labels, sq
 
 
+def _gmm_work(lib, n: int, d: int, k: int, scatter_chunks: int, dev) -> torch.Tensor:
+    wb = int(lib.tip_gmm_work_bytes(n, d, k, scatter_chunks))
+    if wb < 0:
+        raise ValueError(f"Gaussian mixture of {n} x {d} rows with {k} components is not supported: "
+                         f"{lib.tip_last_error().decode(errors='replace')}")
+    return torch.empty(wb, dtype=torch.uint8, device=dev)
+
+
+def gmm_quad(x: torch.Tensor, means: torch.Tensor, prec_chol: torch.Tensor) -> torch.Tensor:
+    """q[k, i] = |(x_i - means_k) . prec_chol_k|^2 (float64 [K, n], fp64 tensor cores) for the [n, d] device matrix
+    x (float32 / float64); means [K, d] and the upper-triangular prec_chol [K, d, d] are float64 on the device."""
+    lib = _lib.load()
+    n, d = x.shape
+    k = means.shape[0]
+    q = torch.empty((k, n), dtype=torch.float64, device=x.device)
+    _lib.check(lib.tip_gmm_quad(_p(x), tip_dtype(x.dtype), n, d, _p(means), _p(prec_chol), k, _p(q), _stream()),
+               "tip_gmm_quad")
+    return q
+
+
+def gmm_log_det(prec_chol: torch.Tensor) -> torch.Tensor:
+    """sklearn _compute_log_det_cholesky ('full'): sum of the logs of the factor's diagonal, per component."""
+    return torch.log(torch.diagonal(prec_chol, dim1=1, dim2=2)).sum(dim=1)
+
+
+def gmm_resp(q: torch.Tensor, d: int, log_weights: torch.Tensor, log_det: torch.Tensor, want_resp: bool = True,
+             want_lse: bool = False, want_labels: bool = False, want_bound: bool = False, work=None):
+    """E-step tail on q [K, n]: (resp [K, n], lse [n], labels [n] int64, lower bound [1]) on the device, each None
+    unless asked for."""
+    lib = _lib.load()
+    k, n = q.shape
+    dev = q.device
+    resp = torch.empty((k, n), dtype=torch.float64, device=dev) if want_resp else None
+    lse = torch.empty(n, dtype=torch.float64, device=dev) if want_lse else None
+    labels = torch.empty(n, dtype=torch.int64, device=dev) if want_labels else None
+    bound = torch.empty(1, dtype=torch.float64, device=dev) if want_bound else None
+    if want_bound and work is None:
+        work = _gmm_work(lib, n, d, k, 0, dev)
+    _lib.check(lib.tip_gmm_resp(_p(q), n, d, k, _p(log_weights), _p(log_det), _p(resp), _p(lse), _p(labels), _p(bound),
+                                _p(work), _stream()), "tip_gmm_resp")
+    return resp, lse, labels, bound
+
+
+def gmm_moments(x: torch.Tensor, resp: torch.Tensor, work=None):
+    """(nk [K], resp^T x [K, d], means [K, d]), float64 on the device (sklearn _estimate_gaussian_parameters)."""
+    lib = _lib.load()
+    n, d = x.shape
+    k = resp.shape[0]
+    if work is None:
+        work = _gmm_work(lib, n, d, k, 0, x.device)
+    nk = torch.empty(k, dtype=torch.float64, device=x.device)
+    sums = torch.empty((k, d), dtype=torch.float64, device=x.device)
+    means = torch.empty((k, d), dtype=torch.float64, device=x.device)
+    _lib.check(lib.tip_gmm_moments(_p(x), tip_dtype(x.dtype), n, d, _p(resp), k, _p(nk), _p(sums), _p(means), _p(work),
+                                   _stream()), "tip_gmm_moments")
+    return nk, sums, means
+
+
+def gmm_scatter(x: torch.Tensor, resp: torch.Tensor, means: torch.Tensor, nk: Optional[torch.Tensor] = None,
+                reg_covar: float = 0.0, scatter_chunks: int = 0, work=None) -> torch.Tensor:
+    """[K, d, d] float64: the weighted scatter matrices S_k (nk None) or the covariances S_k / nk + reg_covar I.
+    scatter_chunks: row chunks of the reduction (0: the library's choice; see gmm_scatter_chunks)."""
+    lib = _lib.load()
+    n, d = x.shape
+    k = resp.shape[0]
+    if work is None:
+        work = _gmm_work(lib, n, d, k, scatter_chunks, x.device)
+    out = torch.empty((k, d, d), dtype=torch.float64, device=x.device)
+    _lib.check(lib.tip_gmm_scatter(_p(x), tip_dtype(x.dtype), n, d, _p(resp), _p(means), k, _p(nk), float(reg_covar),
+                                   int(scatter_chunks), _p(out), _p(work), _stream()), "tip_gmm_scatter")
+    return out
+
+
+def gmm_scatter_chunks(n: int, d: int, k: int, requested: int = 0) -> int:
+    """Row chunks tip_gmm_scatter uses for this shape (requested 0: automatic), after the scratch cap."""
+    return int(_lib.load().tip_gmm_scatter_chunks(n, d, k, requested))
+
+
+GMM_FIT_ERROR = ("Fitting the mixture model failed because some components have ill-defined empirical covariance "
+                 "(for instance caused by singleton or collapsed samples). Try to decrease the number of components, "
+                 "increase reg_covar, or scale the input data.")
+
+
+def gmm_factor(cov: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """sklearn _compute_precision_cholesky ('full') on the device, batched over the components, float64:
+    prec_chol_k = inv(cholesky(cov_k))^T (upper triangular).  Returns (prec_chol [K, d, d], log det [K], info [K]
+    int32: non-zero where cov_k is not positive definite; the caller raises)."""
+    chol, info = torch.linalg.cholesky_ex(cov)
+    eye = torch.eye(cov.shape[-1], dtype=cov.dtype, device=cov.device).expand_as(cov)
+    prec = torch.linalg.solve_triangular(chol, eye, upper=False).transpose(1, 2).contiguous()
+    return prec, gmm_log_det(prec), info
+
+
+def gmm_init(x: torch.Tensor, labels: torch.Tensor, k: int, reg_covar: float, work=None):
+    """sklearn GaussianMixture._initialize from hard labels (one-hot responsibilities, weights = nk / n).
+    Returns (weights, means, covariances, prec_chol, log_det, info) on the device."""
+    if work is None:
+        work = _gmm_work(_lib.load(), x.shape[0], x.shape[1], k, 0, x.device)
+    resp = torch.nn.functional.one_hot(labels.to(torch.int64), k).to(torch.float64).t().contiguous()
+    nk, _, means = gmm_moments(x, resp, work)
+    cov = gmm_scatter(x, resp, means, nk, reg_covar, 0, work)
+    prec, log_det, info = gmm_factor(cov)
+    return nk / x.shape[0], means, cov, prec, log_det, info
+
+
+def _raise_if_failed(info: torch.Tensor, bound: Optional[torch.Tensor] = None):
+    flags = info.to(torch.float64) if bound is None else torch.cat([info.to(torch.float64), bound])
+    h = flags.cpu().numpy()
+    if np.any(h[:info.shape[0]] != 0) or (bound is not None and not np.isfinite(h[-1])):
+        raise ValueError(GMM_FIT_ERROR)
+    return None if bound is None else float(h[-1])
+
+
+def _gmm_step(x, weights, means, prec_chol, log_det, reg_covar, work, ev=None):
+    """One E-step + M-step on device state; returns (bound tensor [1], weights, means, cov, prec, log_det, info)."""
+    d = x.shape[1]
+    mark = (lambda i: ev[i].record()) if ev is not None else (lambda i: None)
+    mark(0)
+    q = gmm_quad(x, means, prec_chol)
+    resp, _, _, bound = gmm_resp(q, d, torch.log(weights), log_det, want_bound=True, work=work)
+    mark(1)
+    nk, sums, new_means = gmm_moments(x, resp, work)
+    weights = nk / nk.sum()
+    cov = gmm_scatter(x, resp, new_means, nk, reg_covar, 0, work)
+    mark(2)
+    prec, new_log_det, info = gmm_factor(cov)
+    mark(3)
+    return bound, weights, new_means, cov, prec, new_log_det, info
+
+
+def gmm_em_step(x: torch.Tensor, weights: torch.Tensor, means: torch.Tensor, prec_chol: torch.Tensor,
+                reg_covar: float):
+    """One sklearn EM iteration (_e_step + _m_step) on the [n, d] device matrix x from the given float64 device
+    state: returns (lower_bound of the E-step, weights, means, covariances, prec_chol) after the M-step.  Raises
+    sklearn's ValueError when a covariance is not positive definite or the bound is not finite."""
+    k = means.shape[0]
+    work = _gmm_work(_lib.load(), x.shape[0], x.shape[1], k, 0, x.device)
+    prec_chol = prec_chol.contiguous()
+    bound, w, mu, cov, prec, _, info = _gmm_step(x, weights.contiguous(), means.contiguous(), prec_chol,
+                                                 gmm_log_det(prec_chol), reg_covar, work)
+    lb = _raise_if_failed(info, bound)
+    return lb, w, mu, cov, prec
+
+
+def gmm_fit(x: torch.Tensor, k: int, max_iter: int = 100, tol: float = 1e-3, reg_covar: float = 1e-6,
+            seed: int = 0, timing: Optional[dict] = None) -> dict:
+    """sklearn GaussianMixture(n_components=k, covariance_type="full", init_params="kmeans", n_init=1).fit on the
+    [n, d] device matrix x: initial responsibilities from the labels of kmeans_fit(x, k, 1, 300, 1e-4, seed), then
+    EM until |lower bound change| < tol or max_iter iterations.  One read-back per iteration (the bound and the
+    factorisation flags).  Returns a dict of device tensors (weights, means, covariances, prec_chol, log_det) and
+    host values (labels_init on the device, n_iter, converged, lower_bound, lower_bounds).
+    timing: a dict that receives CUDA-event milliseconds per phase (kmeans, estep, mstep, factor, total)."""
+    lib = _lib.load()
+    n, d = x.shape
+    work = _gmm_work(lib, n, d, k, 0, x.device)
+    ev = None
+    if timing is not None:
+        new = lambda: torch.cuda.Event(enable_timing=True)
+        t_start, t_km = new(), new()
+        t_start.record()
+    _, labels, _, _ = kmeans_fit(x, k, 1, 300, 1e-4, seed)
+    if timing is not None:
+        t_km.record()
+    weights, means, cov, prec, log_det, info = gmm_init(x, labels, k, reg_covar, work)
+    _raise_if_failed(info)
+    steps = []
+    lower_bound, bounds, converged, n_iter = -np.inf, [], False, 0
+    for n_iter in range(1, max_iter + 1):
+        prev = lower_bound
+        if timing is not None:
+            ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
+            steps.append(ev)
+        bound, weights, means, cov, prec, log_det, info = _gmm_step(x, weights, means, prec, log_det, reg_covar, work, ev)
+        lower_bound = _raise_if_failed(info, bound)
+        bounds.append(lower_bound)
+        if abs(lower_bound - prev) < tol:
+            converged = True
+            break
+    if timing is not None:
+        t_end = torch.cuda.Event(enable_timing=True)
+        t_end.record()
+        torch.cuda.synchronize()
+        timing["kmeans"] = timing.get("kmeans", 0.0) + t_start.elapsed_time(t_km)
+        for key, i in (("estep", 0), ("mstep", 1), ("factor", 2)):
+            timing[key] = timing.get(key, 0.0) + sum(e[i].elapsed_time(e[i + 1]) for e in steps)
+        timing["total"] = timing.get("total", 0.0) + t_start.elapsed_time(t_end)
+    return {"weights": weights, "means": means, "covariances": cov, "prec_chol": prec, "log_det": log_det,
+            "labels_init": labels, "n_iter": n_iter, "converged": converged, "lower_bound": lower_bound,
+            "lower_bounds": bounds}
+
+
 def silhouette_samples(x: torch.Tensor, labels: torch.Tensor, n_clusters: int,
                        span_tiles: Optional[int] = None) -> torch.Tensor:
     """sklearn silhouette_samples of the [n, d] device matrix x (float32 / float64) under labels in
