@@ -38,6 +38,8 @@
  *   tip_gmm_resp        sklearn _estimate_log_prob_resp (logsumexp, exp(log_resp)) and _e_step's mean
  *   tip_gmm_moments     sklearn _estimate_gaussian_parameters: nk = sum(resp) + 10 eps, means = resp.T @ X / nk
  *   tip_gmm_scatter     sklearn _estimate_gaussian_covariances_full: (resp_k * diff.T) @ diff / nk + reg_covar I
+ *   tip_cov_location    src/core/surprise.py:385-386 EmpiricalCovariance().fit: location_ = X.mean(0) and
+ *                       np.cov's float64 centring mean (the scatter reuses tip_gmm_scatter)
  */
 #ifndef B200TIP_H
 #define B200TIP_H
@@ -470,6 +472,15 @@ int tip_gmm_moments(const void* x, int dtype, int64_t n, int64_t d, const double
 int tip_gmm_scatter(const void* x, int dtype, int64_t n, int64_t d, const double* resp,
                     const double* means, int32_t k, const double* nk, double reg_covar,
                     int32_t scatter_chunks, double* out, void* work, void* stream);
+
+/* ---- empirical covariance (sklearn EmpiricalCovariance.fit) --------------------------------------------
+ * tip_cov_location: x n x d (TIP_F32/TIP_F64), 1 <= n < 2^31, 1 <= d <= 65536.  location[d] (x's dtype) =
+ * X.mean(0) bit for bit as NumPy computes it (d >= 2: sequential sum over the rows in x's dtype; d == 1:
+ * NumPy's pairwise sum), divided by n once; mean[d] (double) = the same sum in float64 / n, np.cov's centring
+ * mean.  *flags (device int32, written by the call) = bit 0: some entry is NaN, bit 1: some entry is +-inf.
+ * The scatter of the fit is tip_gmm_scatter with k = 1, unit weights, means = mean and nk = {n}. */
+int tip_cov_location(const void* x, int dtype, int64_t n, int64_t d, void* location, double* mean,
+                     int32_t* flags, void* stream);
 
 /* ---- bring-up / validation: plain accumulator dump ------------------------------------
  * out[256*256] (fp32, row-major, leading dimension 256) = tail-augmented dot products of q rows

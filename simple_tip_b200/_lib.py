@@ -99,6 +99,7 @@ _SIGNATURES = {
     "tip_gmm_resp": (C.c_int, [_vp, _i64, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "tip_gmm_moments": (C.c_int, [_vp, C.c_int, _i64, _i64, _vp, _i32, _vp, _vp, _vp, _vp, _vp]),
     "tip_gmm_scatter": (C.c_int, [_vp, C.c_int, _i64, _i64, _vp, _vp, _i32, _vp, C.c_double, _i32, _vp, _vp, _vp]),
+    "tip_cov_location": (C.c_int, [_vp, C.c_int, _i64, _i64, _vp, _vp, _vp, _vp]),
 }
 
 _lock = threading.Lock()

@@ -108,6 +108,14 @@ def _gmm_backend(backend: Optional[str]) -> str:
     return backend
 
 
+def _cov_backend(backend: Optional[str]) -> str:
+    """backend=None: the B200TIP_COV environment variable, default "sklearn"."""
+    backend = backend if backend is not None else os.environ.get("B200TIP_COV", "sklearn")
+    if backend not in ("sklearn", "device"):
+        raise ValueError(f"backend must be 'sklearn' or 'device', got {backend!r}")
+    return backend
+
+
 def _trace_matrix(activations):
     """[N, D] traces: the device matrix for torch CUDA traces, else the reference's host flattening."""
     from .. import engine as E
@@ -324,16 +332,27 @@ class MDSA(SA):
     """Mahalanobis-distance surprise adequacy (surprise.py:374-393): squared Mahalanobis distance to the mean of
     the training traces.  Fit = sklearn's `EmpiricalCovariance` on the host exactly as in the reference (one
     D x D covariance, its pseudo-inverse); score = whitening by a factor of the precision + squared row norm on
-    the GPU (tip_whiten + tip_row_sqnorm), float64 out like `EmpiricalCovariance.mahalanobis`."""
+    the GPU (tip_whiten + tip_row_sqnorm), float64 out like `EmpiricalCovariance.mahalanobis`.
+    backend="sklearn" (default, or B200TIP_COV unset): the fit is sklearn's on the host.  backend="device": the fit
+    runs on the GPU (core/covariance.py: sklearn's location_ bit for bit, the covariance and its pseudo-inverse in
+    float64); CUDA traces then stay on the device, and the whitening factor comes from the fit's own
+    eigendecomposition over the live columns."""
 
-    def __init__(self, activations: Activations):
+    def __init__(self, activations: Activations, *, backend: Optional[str] = None):
         super().__init__()
-        from sklearn.covariance import EmpiricalCovariance
-
         from .. import engine as E
 
-        host = E.device_matrix(activations)
-        acts = host.cpu().numpy() if host is not None else _flatten_layers(activations)
+        self.backend = _cov_backend(backend)
+        if self.backend == "device":
+            from .covariance import EmpiricalCovariance
+
+            E.require_cuda()
+            acts = _trace_matrix(activations)
+        else:
+            from sklearn.covariance import EmpiricalCovariance
+
+            host = E.device_matrix(activations)
+            acts = host.cpu().numpy() if host is not None else _flatten_layers(activations)
         self.covariance_matrix = EmpiricalCovariance()
         self.covariance_matrix.fit(acts)
         self._width = int(acts.shape[1])
@@ -355,6 +374,8 @@ class MDSA(SA):
         x = _device_rows(activations)
         if x.ndim != 2 or int(x.shape[1]) != self._width:
             raise ValueError(f"X has {tuple(x.shape)[1:]} features, but MDSA was fitted with {self._width} features")
+        if self.backend == "device":
+            return self.covariance_matrix._scores(x).cpu().numpy()
         if self._centres is None:
             self._upload()
         return E.quadratic_forms(x, self._centres)[0].cpu().numpy()

@@ -1,0 +1,159 @@
+// covariance.cu — the N-sized pass of sklearn's EmpiricalCovariance.fit that the Gaussian-mixture kernels do not
+// already cover: the column means.  (The scatter is tip_gmm_scatter with one component and unit weights.)
+//
+// sklearn's `location_ = X.mean(0)` is NumPy's add.reduce over axis 0 in the input dtype, then one division by n.
+// On a C-contiguous [n, d] matrix with d >= 2 that reduce is a sequential sum over the rows, starting from 0; with
+// d == 1 the reduced axis is the contiguous one and NumPy sums it pairwise (numpy/_core/src/umath/loops_utils.h:
+// blocks of <= 128 with eight stride-8 accumulators, larger blocks split at n/2 - (n/2)%8).  `np.cov(X.T)` centres
+// on its own float64 mean, which follows the same two rules in float64.  Both are reproduced here bit for bit:
+//
+//   cov_location_kernel     d >= 2: one thread per column walks the rows in order (8 loads in flight), one
+//                           input-dtype chain and one float64 chain, IEEE adds without contraction
+//   cov_location_1d_kernel  d == 1: one thread, NumPy's pairwise sum in both dtypes
+//
+// The division is done in double and rounded once to the input dtype, which is the correctly rounded quotient for
+// float32 as well (NumPy divides float32 by an intp in double and casts back).  Non-finite inputs set flags bits
+// (1: NaN, 2: +-inf) so that the fit can raise sklearn's error instead of returning NaN.
+#include "common.cuh"
+
+namespace tip {
+
+constexpr int kCovThreads = 32;      // one warp per CTA: d = 1600 gives 50 CTAs, latency-bound chains spread out
+constexpr int kCovUnroll = 8;
+
+__device__ __forceinline__ int cov_flag(double v) {
+  return isnan(v) ? 1 : (isinf(v) ? 2 : 0);
+}
+
+template <typename T>
+__device__ __forceinline__ T cov_div(T s, int64_t n) {
+  return (T)__ddiv_rn((double)s, (double)n);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kCovThreads) cov_location_kernel(const T* __restrict__ x, int64_t n, int64_t d,
+                                                                   T* __restrict__ loc, double* __restrict__ mean,
+                                                                   int32_t* __restrict__ flags) {
+  using R = Rn<T>;
+  const int64_t c = (int64_t)blockIdx.x * kCovThreads + threadIdx.x;
+  if (c >= d) return;
+  T s = (T)0;
+  double s64 = 0.0;
+  int flag = 0;
+  int64_t r = 0;
+  for (; r + kCovUnroll <= n; r += kCovUnroll) {
+    T v[kCovUnroll];
+#pragma unroll
+    for (int u = 0; u < kCovUnroll; u++) v[u] = x[(r + u) * d + c];
+#pragma unroll
+    for (int u = 0; u < kCovUnroll; u++) {
+      s = R::add(s, v[u]);
+      s64 = __dadd_rn(s64, (double)v[u]);
+      flag |= cov_flag((double)v[u]);
+    }
+  }
+  for (; r < n; r++) {
+    const T v = x[r * d + c];
+    s = R::add(s, v);
+    s64 = __dadd_rn(s64, (double)v);
+    flag |= cov_flag((double)v);
+  }
+  loc[c] = cov_div<T>(s, n);
+  mean[c] = __ddiv_rn(s64, (double)n);
+  if (flag) atomicOr(flags, flag);      // an integer flag: the result does not depend on the order
+}
+
+// one leaf (n <= 128) of NumPy's pairwise sum, accumulated in A
+template <typename A, typename T>
+__device__ A cov_leaf(const T* __restrict__ x, int n) {
+  using R = Rn<A>;
+  if (n < 8) {
+    A res = (A)0;
+    for (int i = 0; i < n; i++) res = R::add(res, (A)x[i]);
+    return res;
+  }
+  A r[8];
+#pragma unroll
+  for (int j = 0; j < 8; j++) r[j] = (A)x[j];
+  int i = 8;
+  const int lim = n - (n % 8);
+  for (; i < lim; i += 8)
+#pragma unroll
+    for (int j = 0; j < 8; j++) r[j] = R::add(r[j], (A)x[i + j]);
+  A res = R::add(R::add(R::add(r[0], r[1]), R::add(r[2], r[3])), R::add(R::add(r[4], r[5]), R::add(r[6], r[7])));
+  for (; i < n; i++) res = R::add(res, (A)x[i]);
+  return res;
+}
+
+// NumPy's pairwise sum of x[0, n) accumulated in A, with an explicit stack (depth <= 32 for n < 2^31)
+template <typename A, typename T>
+__device__ A cov_pairwise(const T* __restrict__ x, int n) {
+  if (n <= 128) return cov_leaf<A, T>(x, n);
+  int off[32], len[32];
+  unsigned char phase[32];
+  A vals[32];
+  int sp = 1, vp = 0;
+  off[0] = 0; len[0] = n; phase[0] = 0;
+  while (sp > 0) {
+    const int top = sp - 1;
+    const int o = off[top], l = len[top];
+    if (l <= 128) {
+      vals[vp++] = cov_leaf<A, T>(x + o, l);
+      sp--;
+      continue;
+    }
+    const int n2 = l / 2 - (l / 2) % 8;
+    if (phase[top] == 0) {
+      phase[top] = 1;
+      off[sp] = o; len[sp] = n2; phase[sp] = 0; sp++;
+    } else if (phase[top] == 1) {
+      phase[top] = 2;
+      off[sp] = o + n2; len[sp] = l - n2; phase[sp] = 0; sp++;
+    } else {
+      const A rgt = vals[--vp];
+      const A lft = vals[--vp];
+      vals[vp++] = Rn<A>::add(lft, rgt);
+      sp--;
+    }
+  }
+  return vals[0];
+}
+
+template <typename T>
+__global__ void cov_location_1d_kernel(const T* __restrict__ x, int64_t n, T* __restrict__ loc,
+                                       double* __restrict__ mean, int32_t* __restrict__ flags) {
+  int flag = 0;
+  for (int64_t i = 0; i < n; i++) flag |= cov_flag((double)x[i]);
+  // the reduce adds the pairwise sum to the identity 0 (this also turns a -0 sum into +0, as NumPy does)
+  loc[0] = cov_div<T>(Rn<T>::add((T)0, cov_pairwise<T, T>(x, (int)n)), n);
+  mean[0] = __ddiv_rn(__dadd_rn(0.0, cov_pairwise<double, T>(x, (int)n)), (double)n);
+  *flags = flag;
+}
+
+}  // namespace tip
+
+using namespace tip;
+
+extern "C" int tip_cov_location(const void* x, int dtype, int64_t n, int64_t d, void* location, double* mean,
+                                int32_t* flags, void* stream) {
+  TIP_REQUIRE(dtype == TIP_F32 || dtype == TIP_F64, "dtype must be TIP_F32 or TIP_F64");
+  TIP_REQUIRE(n >= 1 && n < (1LL << 31) && d >= 1 && d <= 65536, "shape");
+  TIP_REQUIRE(x && location && mean && flags, "null pointer");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (d == 1) {
+    if (dtype == TIP_F32)
+      cov_location_1d_kernel<float><<<1, 1, 0, st>>>((const float*)x, n, (float*)location, mean, flags);
+    else
+      cov_location_1d_kernel<double><<<1, 1, 0, st>>>((const double*)x, n, (double*)location, mean, flags);
+    TIP_LAUNCH_CHECK();
+    return TIP_OK;
+  }
+  TIP_CHECK_CUDA(cudaMemsetAsync(flags, 0, sizeof(int32_t), st));
+  const unsigned grid = (unsigned)((d + kCovThreads - 1) / kCovThreads);
+  if (dtype == TIP_F32)
+    cov_location_kernel<float><<<grid, kCovThreads, 0, st>>>((const float*)x, n, d, (float*)location, mean, flags);
+  else
+    cov_location_kernel<double><<<grid, kCovThreads, 0, st>>>((const double*)x, n, d, (double*)location, mean, flags);
+  TIP_LAUNCH_CHECK();
+  return TIP_OK;
+}

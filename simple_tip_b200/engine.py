@@ -1513,6 +1513,89 @@ def gmm_fit(x: torch.Tensor, k: int, max_iter: int = 100, tol: float = 1e-3, reg
             "lower_bounds": bounds}
 
 
+# ------------------------------------------------------------------------------------------
+# MDSA's EmpiricalCovariance (surprise.py:374-393): location, scatter, pseudo-inverse
+# ------------------------------------------------------------------------------------------
+def cov_location(x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """(location [d] x.dtype = NumPy's x.mean(0) bit for bit, np.cov's float64 centring mean [d], non-finite flags
+    [1] int32: bit 0 NaN, bit 1 inf) of the [n, d] device matrix x, all on the device."""
+    lib = _lib.load()
+    n, d = x.shape
+    loc = torch.empty(d, dtype=x.dtype, device=x.device)
+    mean = torch.empty(d, dtype=torch.float64, device=x.device)
+    flags = torch.empty(1, dtype=torch.int32, device=x.device)
+    _lib.check(lib.tip_cov_location(_p(x), tip_dtype(x.dtype), n, d, _p(loc), _p(mean), _p(flags), _stream()),
+               "tip_cov_location")
+    return loc, mean, flags
+
+
+def cov_fit(x: torch.Tensor, timing: Optional[dict] = None) -> dict:
+    """sklearn EmpiricalCovariance().fit on the [n, d] device matrix x (float32 / float64), n >= 1:
+    - location = x.mean(0) in x's dtype (bit for bit), covariance = np.cov(x.T, bias=1) in float64: the DMMA
+      scatter of tip_gmm_scatter (k = 1, unit weights) centred on the float64 mean, divided by n;
+    - live columns: those with a non-zero diagonal.  A column whose centred values are all exactly 0 has an exactly
+      zero row and column; it is left out of the eigendecomposition (its eigenvalue, 0, is one scipy drops too);
+    - precision = scipy's pinvh of the live block: torch.linalg.eigh in float64, eigenvalues kept where
+      |s| > d * eps * max|s| (d: all columns), (U / s) @ U^T; zero on dead rows and columns;
+    - the scoring factor W [d_live, d_live] float32 = U diag(s^-1/2) over the kept s > 0 (zero columns after them),
+      so that |(x[:, live] - location[live]) . W|^2 is the Mahalanobis form of the precision.
+    Raises sklearn's ValueError on NaN / inf input (one read-back).  Returns device tensors: location, mean,
+    covariance, live (int64), eigenvalues (of the live block), rank (host int), precision, score_mu (float64
+    location[live]), score_w (None when d_live == 0).  timing: receives CUDA-event milliseconds (cov_location,
+    scatter, eigh, total)."""
+    n, d = x.shape
+    ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)] if timing is not None else None
+    if ev:
+        ev[0].record()
+    loc, mean, flags = cov_location(x)
+    if ev:
+        ev[1].record()
+    f = int(flags.item())
+    if f & 1:
+        raise ValueError("Input X contains NaN.")
+    if f & 2:
+        raise ValueError(f"Input X contains infinity or a value too large for {np.dtype(NP_DTYPE[x.dtype])!r}.")
+    ones = torch.ones((1, n), dtype=torch.float64, device=x.device)
+    nk = torch.full((1,), float(n), dtype=torch.float64, device=x.device)
+    cov = gmm_scatter(x, ones, mean.reshape(1, d), nk, 0.0)[0]
+    if ev:
+        ev[2].record()
+    live = torch.nonzero(torch.diagonal(cov) != 0).flatten()
+    dl = int(live.shape[0])
+    precision = torch.zeros((d, d), dtype=torch.float64, device=x.device)
+    score_w, rank = None, 0
+    s = torch.empty(0, dtype=torch.float64, device=x.device)
+    if dl:
+        s, u = torch.linalg.eigh(cov.index_select(0, live).index_select(1, live))
+        cutoff = d * np.finfo(np.float64).eps * s.abs().max()
+        keep = s.abs() > cutoff
+        uk, sk = u[:, keep], s[keep]
+        rank = int(sk.shape[0])
+        block = (uk * (1.0 / sk)) @ uk.t()
+        precision[live.unsqueeze(1), live.unsqueeze(0)] = block
+        pos = sk > 0
+        score_w = torch.zeros((dl, dl), dtype=torch.float32, device=x.device)
+        score_w[:, :int(pos.sum())] = (uk[:, pos] * sk[pos].rsqrt()).to(torch.float32)
+    if ev:
+        ev[3].record()
+        torch.cuda.synchronize()
+        for key, i in (("cov_location", 0), ("scatter", 1), ("eigh", 2)):
+            timing[key] = timing.get(key, 0.0) + ev[i].elapsed_time(ev[i + 1])
+        timing["total"] = timing.get("total", 0.0) + ev[0].elapsed_time(ev[3])
+    return {"location": loc, "mean": mean, "covariance": cov, "live": live, "eigenvalues": s, "rank": rank,
+            "precision": precision, "score_mu": mean.new_empty(0) if not dl else
+            loc.index_select(0, live).to(torch.float64), "score_w": score_w}
+
+
+def cov_scores(x: torch.Tensor, fit: dict) -> torch.Tensor:
+    """Squared Mahalanobis distances [m] (float64, device) of the rows of x to a cov_fit: fp32 whitening of the
+    live columns (tip_whiten) + double row norms; zeros when no column is live."""
+    if fit["score_w"] is None:
+        return torch.zeros(x.shape[0], dtype=torch.float64, device=x.device)
+    cols = fit["live"].to(torch.int32)
+    return quadratic_forms(x, [(fit["score_mu"], fit["score_w"])], cols)[0]
+
+
 def silhouette_samples(x: torch.Tensor, labels: torch.Tensor, n_clusters: int,
                        span_tiles: Optional[int] = None) -> torch.Tensor:
     """sklearn silhouette_samples of the [n, d] device matrix x (float32 / float64) under labels in
