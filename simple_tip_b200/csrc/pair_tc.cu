@@ -18,9 +18,14 @@
 // wgmma accumulator layout the four lanes of a quad hold one row between them (8 of every 32
 // consecutive columns each), so the per-row reductions finish with two quad shuffles.  The two
 // consumer warpgroups drift out of phase, so one's MMAs overlap the other's reduction.
-// Pipeline: kStages-deep shared-memory ring (full/empty mbarriers, TMA -> wgmma).  Resident-query
-// variant (RESA, short packed rows): the query tile's K chunks are loaded once per work item and
-// the ring carries train chunks only.
+// Pipeline: kStages-deep shared-memory ring (full/empty mbarriers, TMA -> wgmma), one wgmma commit
+// group per K chunk.  Streaming variant: each group is waited for and its stage released before the
+// next chunk.  Resident-query variant (RESA, short packed rows): the query tile's K chunks are loaded
+// once per run of consecutive work items on the same query tile, the ring carries train chunks only,
+// a tile's groups are committed before one wait, and the tile's stages are released after it.
+// ptxas still serialises the wgmma of the MODE_NN kernels (C7520, a data-dependent branch with side
+// effects in the tile loop: the candidate staging), so there the groups do not overlap; the epilogue
+// never overlaps its own warpgroup's MMAs.
 #include <cuda.h>
 #include <cudaTypedefs.h>
 
@@ -135,6 +140,12 @@ __device__ __forceinline__ uint64_t smem_desc(uint32_t addr) {
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// Operand fence: the compiler may not move any access to the accumulator registers across this point, so
+// reads happen after the wait that retires the MMAs and never while an MMA that writes them is in flight.
+__device__ __forceinline__ void acc_fence(float (&d)[64]) {
+#pragma unroll
+  for (int i = 0; i < 64; i++) asm volatile("" : "+f"(d[i])::"memory");
+}
 
 #define TIP_ACC8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), \
                     "+f"(d[i + 6]), "+f"(d[i + 7])
@@ -366,6 +377,7 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     if (lane == 0) {
       int stage = 0;
       uint32_t phase = 0, a_phase = 0;
+      int a_row0 = -1;    // query tile in shared memory (RESA): consecutive items of the same tile reuse it
       long long n_tiles_done = 0, n_items_done = 0;
       int w_static = blockIdx.x;
       for (int k = 0;; k++) {
@@ -384,11 +396,14 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         const int ntiles = (it.col1 - it.col0 + BN - 1) / BN;
         if (ntiles <= 0) continue;   // padding entry of a balanced work list
         n_tiles_done += ntiles; n_items_done++;
-        if (RESA) {
-          mbar_wait(a_empty, a_phase ^ 1u);      // the previous item's MMAs have retired (first item: passes at once)
+        if (RESA && it.q_row0 != a_row0) {
+          // the consumers arrive once they start an item of another query tile, when every MMA on this one has
+          // retired (first load: passes at once)
+          mbar_wait(a_empty, a_phase ^ 1u);
           mbar_expect_tx(a_full, (uint32_t)nchunks * kABytes);
           for (int c = 0; c < nchunks; c++) tma_load_2d(base + (uint32_t)c * kABytes, &tmA, a_full, c * BK, it.q_row0);
           a_phase ^= 1u;
+          a_row0 = it.q_row0;
         }
         for (int t = 0; t < ntiles; t++) {
           TL(8);
@@ -419,7 +434,7 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     __syncwarp();
   } else if (warp >= 4) {
     // ================= consumers: wgmma + register epilogue =================
-    const int cw = warp - 4;                      // consumer warp 0..7
+    const int cw = warp - 4;                    // consumer warp 0..7
     const int g = cw >> 2;                        // consumer warpgroup: query rows [64 g, 64 g + 64)
     const int sub = lane & 3;
     const unsigned qmask = 0xFu << (lane & 28);   // the lanes of this quad
@@ -432,9 +447,11 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     sh.cand_mask = reinterpret_cast<uint32_t*>(sh.cand_col + kCandSlots * BM);
     const float kInf = __int_as_float(0x7f800000);
     float acc[64];
-    int stage = 0;
+    int stage = 0, rel_stage = 0;  // next stage to consume / to release
     uint32_t phase = 0, a_phase = 0;
+    int a_row0 = -1;
     bool first_item = true;
+    int tl_tile0 = 0;           // timeline index of the item's first tile
     for (int k = 0;; k++) {
       const int slot = k & 1;
       mbar_wait(sched_full(slot), (uint32_t)(k >> 1) & 1u);
@@ -480,42 +497,66 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
           if (s.valid_row) s.thr = nn_threshold(s.s_ref, s.nx, s.e2, s.g);
         }
       }
-      if (RESA) {
+      if (RESA && it.q_row0 != a_row0) {
+        // another query tile: every MMA on the previous one has retired (the tile loop drains), hand its buffer back
+        if (a_row0 >= 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(a_empty);
+        }
         mbar_wait(a_full, a_phase);
         a_phase ^= 1u;
+        a_row0 = it.q_row0;
       }
       const bool dump_item = MODE == MODE_DUMP && first_item && blockIdx.x == 0;
       first_item = false;
 
-      for (int t = 0; t < ntiles; t++) {
-        if (cw == 0 && lane == 0) TL(0);
+#define TLT(t, slot)                                                                                      \
+  do {                                                                                                    \
+    if (cw == 0 && lane == 0 && args.timeline && blockIdx.x == 0 && tl_tile0 + (t) < args.timeline_tiles) \
+      args.timeline[(int64_t)(tl_tile0 + (t)) * 16 + (slot)] = clock64();                                 \
+  } while (0)
+
+      // Resident query tile: issue the MMAs of tile t into acc, one commit group per K chunk, all of them in flight
+      // before the first wait; retire_tile waits and releases their stages.
+      auto issue_tile = [&](int t) {
+        TLT(t, 0);
         for (int c = 0; c < nchunks; c++) {
           mbar_wait(full_bar(stage), phase);
-          const uint32_t a_addr = (RESA ? base + (uint32_t)c * kABytes : base + stage * kStageBytes) + (uint32_t)g * 64 * 128;
-          const uint32_t b_addr = RESA ? b_ring + (uint32_t)stage * kBBytes : base + stage * kStageBytes + kABytes;
+          const uint32_t a_addr = base + (uint32_t)c * kABytes + (uint32_t)g * 64 * 128;
+          const uint32_t b_addr = b_ring + (uint32_t)stage * kBBytes;
           const uint64_t adesc = smem_desc(a_addr), bdesc = smem_desc(b_addr);
           const int nm = min(4, k16 - 4 * c);
+          acc_fence(acc);
           wgmma_fence();
           wgmma_m64n128k16<F16>(acc, adesc, bdesc, c > 0 ? 1u : 0u);
           for (int kk = 1; kk < nm; kk++) wgmma_m64n128k16<F16>(acc, adesc + 2u * kk, bdesc + 2u * kk, 1u);
           wgmma_commit();
-          wgmma_wait_all();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(empty_bar(stage));
+          acc_fence(acc);
           if (++stage == kStages) { stage = 0; phase ^= 1u; }
         }
-        if (cw == 0 && lane == 0) TL(1);
-
-        const int col_base = it.col0 + t * BN;
-        const bool partial = col_base + BN > it.col1;
-        float seen[2];
+      };
+      // Wait for every MMA in flight (the tile in acc), then release the stages not released yet.
+      auto retire_tile = [&](int t, int n_release) {
+        wgmma_wait_all();
+        acc_fence(acc);
+        __syncwarp();
+        for (int c = 0; c < n_release; c++) {
+          if (lane == 0) mbar_arrive(empty_bar(rel_stage));
+          if (++rel_stage == kStages) rel_stage = 0;
+        }
+        TLT(t, 1);
+      };
+      // The shared running minimum of the rows, read before the wait on the MMAs and used after the epilogue.
+      auto load_seen = [&](uint32_t (&sb)[2]) {
 #pragma unroll
         for (int h = 0; h < 2; h++) {
-          uint32_t b = 0x7f800000u;
-          if (MODE == MODE_NN && st[h].valid_row && sub == 0) b = ld_volatile_u32(args.row_min_bits + st[h].row);
-          if (MODE == MODE_NN) b = __shfl_sync(0xffffffffu, b, lead);
-          seen[h] = __uint_as_float(b);
+          sb[h] = 0x7f800000u;
+          if (MODE == MODE_NN && st[h].valid_row && sub == 0) sb[h] = ld_volatile_u32(args.row_min_bits + st[h].row);
         }
+      };
+      auto epilogue = [&](int t, const uint32_t (&sb)[2]) {
+        const int col_base = it.col0 + t * BN;
+        const bool partial = col_base + BN > it.col1;
         if (MODE == MODE_DUMP) {
           if (dump_item && t < 2) {     // the first 128 rows x 256 columns of the first item
 #pragma unroll
@@ -525,17 +566,32 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             }
           }
         } else {
+          bool any = true;
+          if (MODE == MODE_NN) {
+            // thr is the same in the four lanes of a quad, so the quad's minimum lies inside the window exactly when
+            // some lane's own minimum does: a tile without any such value changes no state and skips the chunk pass.
+            // Masking (partial tile, excluded class) only raises values, so the unmasked minimum decides safely.
+            float m[2] = {kInf, kInf};
 #pragma unroll
-          for (int c = 0; c < BN / 32; c++) {
+            for (int i = 0; i < 64; i += 4) {
+              m[0] = fminf(m[0], fminf(acc[i], acc[i + 1]));
+              m[1] = fminf(m[1], fminf(acc[i + 2], acc[i + 3]));
+            }
+            any = __any_sync(0xffffffffu, (st[0].valid_row && m[0] <= st[0].thr) || (st[1].valid_row && m[1] <= st[1].thr));
+          }
+          if (any) {
 #pragma unroll
-            for (int h = 0; h < 2; h++) {
-              float v[8];
+            for (int c = 0; c < BN / 32; c++) {
 #pragma unroll
-              for (int jj = 0; jj < 4; jj++) {
-                v[2 * jj] = acc[4 * (4 * c + jj) + 2 * h];
-                v[2 * jj + 1] = acc[4 * (4 * c + jj) + 2 * h + 1];
+              for (int h = 0; h < 2; h++) {
+                float v[8];
+#pragma unroll
+                for (int jj = 0; jj < 4; jj++) {
+                  v[2 * jj] = acc[4 * (4 * c + jj) + 2 * h];
+                  v[2 * jj + 1] = acc[4 * (4 * c + jj) + 2 * h + 1];
+                }
+                epi_chunk<MODE, EXCL>(args, st[h], sh, v, col_base + 32 * c, sub, qmask, partial, row_h0 + 8 * h);
               }
-              epi_chunk<MODE, EXCL>(args, st[h], sh, v, col_base + 32 * c, sub, qmask, partial, row_h0 + 8 * h);
             }
           }
         }
@@ -543,22 +599,100 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 #pragma unroll
           for (int h = 0; h < 2; h++) {
             EpiState& s = st[h];
+            const float seen = __uint_as_float(__shfl_sync(0xffffffffu, sb[h], lead));
             if (!s.valid_row) continue;
             // share the running minimum across everybody scanning other columns for the same query
             const float mine = fmaxf(s.best + s.nx, 0.f);
-            if (sub == 0 && mine < seen[h]) atomicMin(args.row_min_bits + s.row, __float_as_uint(mine));
-            if (seen[h] < s.s_ref) {
-              s.s_ref = seen[h];
+            if (sub == 0 && mine < seen) atomicMin(args.row_min_bits + s.row, __float_as_uint(mine));
+            if (seen < s.s_ref) {
+              s.s_ref = seen;
               s.thr = nn_threshold(s.s_ref, s.nx, s.e2, s.g);
             }
           }
         }
-        if (cw == 0 && lane == 0) { TL(7); tl_tile++; }
-      }
+        TLT(t, 7);
+      };
+
       if (RESA) {
-        __syncwarp();
-        if (lane == 0) mbar_arrive(a_empty);     // every wgmma of this item has completed (waited above)
+        for (int t = 0; t < ntiles; t++) {
+          uint32_t sb[2];
+          issue_tile(t);
+          load_seen(sb);
+          retire_tile(t, nchunks);
+          epilogue(t, sb);
+        }
+      } else {
+        // streaming (wide rows, many chunks per tile): the MMA loop dominates; each chunk is retired before the next
+        for (int t = 0; t < ntiles; t++) {
+          TLT(t, 0);
+          for (int c = 0; c < nchunks; c++) {
+            mbar_wait(full_bar(stage), phase);
+            const uint32_t a_addr = base + stage * kStageBytes + (uint32_t)g * 64 * 128;
+            const uint32_t b_addr = base + stage * kStageBytes + kABytes;
+            const uint64_t adesc = smem_desc(a_addr), bdesc = smem_desc(b_addr);
+            const int nm = min(4, k16 - 4 * c);
+            wgmma_fence();
+            wgmma_m64n128k16<F16>(acc, adesc, bdesc, c > 0 ? 1u : 0u);
+            for (int kk = 1; kk < nm; kk++) wgmma_m64n128k16<F16>(acc, adesc + 2u * kk, bdesc + 2u * kk, 1u);
+            wgmma_commit();
+            wgmma_wait_all();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(empty_bar(stage));
+            if (++stage == kStages) { stage = 0; phase ^= 1u; }
+          }
+          TLT(t, 1);
+          const int col_base = it.col0 + t * BN;
+          const bool partial = col_base + BN > it.col1;
+          float seen[2];
+#pragma unroll
+          for (int h = 0; h < 2; h++) {
+            uint32_t b = 0x7f800000u;
+            if (MODE == MODE_NN && st[h].valid_row && sub == 0) b = ld_volatile_u32(args.row_min_bits + st[h].row);
+            if (MODE == MODE_NN) b = __shfl_sync(0xffffffffu, b, lead);
+            seen[h] = __uint_as_float(b);
+          }
+          if (MODE == MODE_DUMP) {
+            if (dump_item && t < 2) {     // the first 128 rows x 256 columns of the first item
+#pragma unroll
+              for (int i = 0; i < 64; i++) {
+                const int col = t * BN + 8 * (i >> 2) + 2 * sub + (i & 1);
+                args.dump[(int64_t)(row_h0 + 8 * ((i >> 1) & 1)) * 256 + col] = acc[i];
+              }
+            }
+          } else {
+#pragma unroll
+            for (int c = 0; c < BN / 32; c++) {
+#pragma unroll
+              for (int h = 0; h < 2; h++) {
+                float v[8];
+#pragma unroll
+                for (int jj = 0; jj < 4; jj++) {
+                  v[2 * jj] = acc[4 * (4 * c + jj) + 2 * h];
+                  v[2 * jj + 1] = acc[4 * (4 * c + jj) + 2 * h + 1];
+                }
+                epi_chunk<MODE, EXCL>(args, st[h], sh, v, col_base + 32 * c, sub, qmask, partial, row_h0 + 8 * h);
+              }
+            }
+          }
+          if (MODE == MODE_NN) {
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+              EpiState& s = st[h];
+              if (!s.valid_row) continue;
+              // share the running minimum across everybody scanning other columns for the same query
+              const float mine = fmaxf(s.best + s.nx, 0.f);
+              if (sub == 0 && mine < seen[h]) atomicMin(args.row_min_bits + s.row, __float_as_uint(mine));
+              if (seen[h] < s.s_ref) {
+                s.s_ref = seen[h];
+                s.thr = nn_threshold(s.s_ref, s.nx, s.e2, s.g);
+              }
+            }
+          }
+          TLT(t, 7);
+        }
       }
+      tl_tile0 += ntiles;
+#undef TLT
 
 #pragma unroll
       for (int h = 0; h < 2; h++) {
