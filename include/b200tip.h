@@ -391,7 +391,11 @@ int tip_kde_lse_f16(const void* q_pack, int64_t m, const void* t_pack, int64_t n
 int tip_pair_prep_f16(const void* src, int dtype, int64_t rows, int64_t d, const float* center, int role,
                       float norm_coef, float norm_scale, void* dst_f16, float* sqnorm, int32_t* flags,
                       void* stream);
-/* merges `slots` partials per row in ascending slot order: out_max, out_sum (fp32) */
+/* merges `slots` partials per row into out_max, out_sum (fp32), in two levels: slot s goes to group s mod 8; each of
+ * the 8 groups merges its slots online in ascending slot order (a higher max rescales the group's sum by
+ * expf(old - new), a lower one adds part_sum * expf(part_max - max)); then the groups are merged in ascending group
+ * order: out_max = the largest group max, out_sum = sum of group sum * expf(group max - out_max).  Slots whose
+ * part_max is -inf (or NaN) are skipped; a row without any other slot gets (-inf, 0). */
 int tip_kde_combine(const float* part_max, const float* part_sum, int64_t m, int32_t slots,
                     float* out_max, float* out_sum, void* stream);
 

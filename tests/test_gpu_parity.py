@@ -991,13 +991,20 @@ def test_lsa_fast_pass_is_verified_and_falls_back():
     _close(out, np_oracle.lsa_oracle(xs, xt))
     chk = lo.kde.last_fast_check
     assert lo.kde.last_operands == "split-bf16 x3" or chk["max_rel_diff"] <= 4e-5, chk
-    # values beyond fp16's range disable the fast operand at fit time / raise the overflow flag at score time
-    big = LSA(xtr * 3.0e4)
-    assert big.kde._engine.fast_ok in (False, True)
+    # queries beyond fp16's range raise the overflow flag at score time: the check rejects the fast pass, retires it
+    # for this KDE, and the call returns exactly what the three-segment pass gives.  (The fit-time range check cannot
+    # trip through LSA, whose whitening removes the scale of the training set: tests/test_gpu_kde_reference.py.)
     far = xte.copy()
     far[:5] *= 1.0e6
-    res = LSA(xtr)(far)
-    assert np.isinf(res[:5]).all() or np.isfinite(res[5:]).all()
+    sa_far = LSA(xtr)
+    assert sa_far.kde._engine.fast_ok
+    res = sa_far(far)
+    assert sa_far.kde.last_fast_check["accepted"] is False, sa_far.kde.last_fast_check
+    assert sa_far.kde._engine.fast_ok is False
+    assert np.all(res[:5] == np.inf), res[:5]
+    slow = sa_far(far)
+    assert sa_far.kde.last_operands == "split-bf16 x3"
+    assert np.array_equal(res.view(np.int64), slow.view(np.int64))
     _close(res[5:][sub[sub >= 5] - 5], np_oracle.lsa_oracle(xtr, far[5:][sub[sub >= 5] - 5]))
 
 
