@@ -12,20 +12,26 @@
 //             silhouette_samples); the query's own column contributes 0
 //   MODE_DUMP raw accumulator tile (bring-up / validation)
 //
-// Roles (384 threads): warpgroup 0 = TMA producer and work-item hand-out (one lane); warpgroups 1
-// and 2 = consumers.  Consumer warpgroup g owns query rows [64 g, 64 g + 64) of the tile: it issues
-// m64n128k16 wgmma for them, keeps the accumulator in registers and reduces it there.  In the
-// wgmma accumulator layout the four lanes of a quad hold one row between them (8 of every 32
-// consecutive columns each), so the per-row reductions finish with two quad shuffles.  The two
-// consumer warpgroups drift out of phase, so one's MMAs overlap the other's reduction.
-// Pipeline: kStages-deep shared-memory ring (full/empty mbarriers, TMA -> wgmma), one wgmma commit
-// group per K chunk.  Streaming variant: each group is waited for and its stage released before the
-// next chunk.  Resident-query variant (RESA, short packed rows): the query tile's K chunks are loaded
-// once per run of consecutive work items on the same query tile, the ring carries train chunks only,
-// a tile's groups are committed before one wait, and the tile's stages are released after it.
-// ptxas still serialises the wgmma of the MODE_NN kernels (C7520, a data-dependent branch with side
-// effects in the tile loop: the candidate staging), so there the groups do not overlap; the epilogue
-// never overlaps its own warpgroup's MMAs.
+// Roles (384 threads): warpgroup 0 = TMA producer and work-item hand-out (one lane of warp 0) and, in
+// the resident MODE_NN kernel, three drain warps; warpgroups 1 and 2 = consumers.  Consumer warpgroup g owns query rows
+// [64 g, 64 g + 64) of the tile: it issues m64n128k16 wgmma for them, keeps the accumulator in
+// registers and reduces it there.  In the wgmma accumulator layout the four lanes of a quad hold one
+// row between them (8 of every 32 consecutive columns each), so the per-row reductions finish with two
+// quad shuffles.  The two consumer warpgroups drift out of phase, so one's MMAs overlap the other's
+// reduction.
+// Pipeline: kStages-deep shared-memory ring (full/empty mbarriers, TMA -> wgmma).  Streaming variant:
+// one commit group per K chunk, each waited for and its stage released before the next chunk.
+// Resident-query variant (RESA, short packed rows): the query tile's K chunks are loaded once per run
+// of consecutive work items on the same query tile, the ring carries train chunks only, and a tile's
+// MMAs form one commit group whose stages are released after its wait.
+// MODE_NN events, resident variant: a consumer quad that finds a chunk inside its row's window only
+// updates its running minimum and writes one record into the tile's mailbox (two, by tile parity, with
+// full/empty mbarriers); the drain warps own the per-row candidate staging (compaction, direct emission
+// when full, the flush at the end of an item).  With no data-dependent staging or divergent shuffles in
+// the consumers' tile loop, ptxas keeps the wgmma asynchronous: a tile's HGMMAs issue back to back.
+// Streaming variant: the quad's first lane stages its events itself; there ptxas still serialises the
+// wgmma (C7520), which costs little next to the per-chunk waits, and moving the staging to the drain
+// warps made the C5 slice slower (DESIGN.md §8).
 #include <cuda.h>
 #include <cudaTypedefs.h>
 
@@ -48,8 +54,20 @@ constexpr int kConsumerWarps = 8;            // two consumer warpgroups
 constexpr int kThreads = 128 + 32 * kConsumerWarps;
 constexpr int kCandSlots = 8;   // per-query staging slots for candidates (MODE_NN)
 constexpr int kCandBytes = kCandSlots * BM * 12;   // value, chunk start, 32-bit column mask
+constexpr int kEvSlots = BN / 32;   // MODE_NN events per row and tile: one per 32-column chunk
+constexpr int kDrainWarps = 3;      // warps 1..3 of warpgroup 0
+// MODE_NN event mailbox, one per tile parity: the consumers record a tile's events, the drain warps stage them
+struct EvRecord { int col; uint32_t mask; float mn, thr; };   // chunk start, column mask, chunk minimum, row thr
+struct EvRow { float thr; int ev; };                          // row thr after the tile, bit c = event in chunk c
+struct EvBuf {
+  EvRecord rec[BM * kEvSlots];
+  EvRow row[BM];
+  int q_row0, flags, pad[2];
+};
+enum { kEvLast = 1, kEvStop = 2 };   // EvBuf::flags: last tile of the item (flush), no more tiles
+constexpr int kEvBytes = 2 * (int)sizeof(EvBuf);
 constexpr int kBarBytes = 256;
-constexpr int kSmemBytes = kRingBytes + 1024 /*align slack*/ + kBarBytes + kCandBytes;
+constexpr int kSmemBytes = kRingBytes + 1024 /*align slack*/ + kBarBytes + kCandBytes + kEvBytes;
 constexpr int kSmemMax = 232448;   // 227 KB per block on sm_90
 static_assert(kResAChunks * kABytes + kStages * kBBytes <= kRingBytes, "resident-query layout does not fit");
 static_assert(kSmemBytes <= kSmemMax, "pair kernel does not fit");
@@ -191,15 +209,60 @@ struct EpiState {
   int col1;
   int ex_lo, ex_hi;                    // train rows this query must ignore (its own class), or empty
   float nx, e2, g, best, thr, s_ref;   // MODE_NN (identical in the four lanes of the row's quad)
-  int n_staged;                        // MODE_NN, kept by the quad's first lane only
+  int n_staged;                        // MODE_NN streaming variant, kept by the quad's first lane only
   float run_max, run_sum;              // MODE_LSE
   double dsum;                         // MODE_DSUM
 };
+// MODE_NN per-row candidate staging: slot k of local row r at [k * BM + r]
 struct EpiShared {
   float* cand_val;
   int* cand_col;
   uint32_t* cand_mask;
 };
+
+// Stage chunk `col` (minimum mn, column mask) of a row with n staged chunks.  Full slots are first compacted against
+// thr (the row's current threshold); if they all stay live, the chunk goes straight to the row's list.
+__device__ __forceinline__ void stage_chunk(const PairArgs& args, const EpiShared& sh, int r, int& n, int64_t row,
+                                            int col, uint32_t mask, float mn, float thr) {
+  if (n == kCandSlots) {
+    int keep = 0;
+    for (int k = 0; k < kCandSlots; k++) {
+      const float sv = sh.cand_val[k * BM + r];
+      if (sv <= thr) {
+        sh.cand_val[keep * BM + r] = sv;
+        sh.cand_col[keep * BM + r] = sh.cand_col[k * BM + r];
+        sh.cand_mask[keep * BM + r] = sh.cand_mask[k * BM + r];
+        keep++;
+      }
+    }
+    n = keep;
+  }
+  if (n < kCandSlots) {
+    sh.cand_val[n * BM + r] = mn;
+    sh.cand_col[n * BM + r] = col;
+    sh.cand_mask[n * BM + r] = mask;
+    n++;
+  } else {
+    const int pos = atomicAdd(args.cand_cnt + row, 1);
+    if (pos < args.cap) {
+      args.cand_idx[(row * args.cap + pos) * 2] = col;
+      args.cand_idx[(row * args.cap + pos) * 2 + 1] = (int)mask;
+    }
+  }
+}
+// End of an item: emit the staged chunks of a row that survive its final threshold.
+__device__ __forceinline__ void flush_row(const PairArgs& args, const EpiShared& sh, int r, int n, int64_t row,
+                                          float thr) {
+  for (int q = 0; q < n; q++) {
+    if (sh.cand_val[q * BM + r] <= thr) {
+      const int pos = atomicAdd(args.cand_cnt + row, 1);
+      if (pos < args.cap) {
+        args.cand_idx[(row * args.cap + pos) * 2] = sh.cand_col[q * BM + r];
+        args.cand_idx[(row * args.cap + pos) * 2 + 1] = (int)sh.cand_mask[q * BM + r];
+      }
+    }
+  }
+}
 
 __device__ __forceinline__ float fast_exp2(float x) {
   float y;
@@ -216,63 +279,61 @@ __device__ __forceinline__ uint32_t ld_volatile_u32(const uint32_t* p) {
 // Reduce the 32 accumulator columns [cbase, cbase + 32) of one query row.  The row's quad holds them:
 // lane `sub` (0..3) has v[2 jj + e] = column cbase + 8 jj + 2 sub + e.  Every lane of the warp calls
 // this (the quad shuffles need the whole warp); the running state comes out the same in the four lanes
-// of a quad, and the quad's first lane alone stages and emits candidates (etid = the row's staging column).
-template <int MODE, bool EXCL>
-__device__ __forceinline__ void epi_chunk(const PairArgs& args, EpiState& st, const EpiShared& sh, float (&v)[8],
-                                          int cbase, int sub, unsigned qmask, bool partial, int etid) {
+// of a quad.  MODE_NN, resident variant: an event (a value inside the row's window) only sets bit c of `ev` and,
+// from the quad's first lane, writes the row's record for chunk c of the tile (rec); the drain warps stage and emit
+// it.  Keeping data-dependent staging out of this loop is what lets ptxas leave the wgmma asynchronous (no C7520).
+// Streaming variant (its MMAs are waited for chunk by chunk anyway): the quad's first lane stages the event itself
+// (etid = the row's staging column).
+template <int MODE, bool EXCL, bool RESA>
+__device__ __forceinline__ void epi_chunk(const PairArgs& args, EpiState& st, const EpiShared& sh, EvRecord* rec,
+                                          int& ev, float (&v)[8], int cbase, int c, int sub, bool partial, int etid) {
   const float kInf = __int_as_float(0x7f800000);
   if (MODE == MODE_NN) {
     if (partial || (EXCL && cbase < st.ex_hi && cbase + 32 > st.ex_lo)) {
       // rare: the chunk runs past the span, or overlaps the train rows this query must ignore
 #pragma unroll
       for (int k = 0; k < 8; k++) {
-        const int c = cbase + 8 * (k >> 1) + 2 * sub + (k & 1);
-        if (c >= st.col1 || (EXCL && c >= st.ex_lo && c < st.ex_hi)) v[k] = kInf;
+        const int col = cbase + 8 * (k >> 1) + 2 * sub + (k & 1);
+        if (col >= st.col1 || (EXCL && col >= st.ex_lo && col < st.ex_hi)) v[k] = kInf;
       }
     }
     float mn = fminf(fminf(fminf(v[0], v[1]), fminf(v[2], v[3])), fminf(fminf(v[4], v[5]), fminf(v[6], v[7])));
     mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, 1));
     mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, 2));
-    if (st.valid_row && mn <= st.thr && mn < kInf) {
-      // event: this chunk holds a value inside the acceptance window of this query (quad-uniform)
-      if (mn < st.best) {
-        st.best = mn;
-        st.s_ref = fminf(st.s_ref, fmaxf(st.best + st.nx, 0.f));
-        st.thr = nn_threshold(st.s_ref, st.nx, st.e2, st.g);
-      }
-      // exact per-column mask of the chunk: the re-rank then touches only rows inside the window
-      uint32_t mask = 0;
+    // event: this chunk holds a value inside the acceptance window of this query (quad-uniform)
+    const bool event = st.valid_row && mn <= st.thr && mn < kInf;
+    if (!RESA) {
+      if (event) {
+        if (mn < st.best) {
+          st.best = mn;
+          st.s_ref = fminf(st.s_ref, fmaxf(st.best + st.nx, 0.f));
+          st.thr = nn_threshold(st.s_ref, st.nx, st.e2, st.g);
+        }
+        const unsigned qmask = 0xFu << ((threadIdx.x & 31) & 28);   // the lanes of this quad
+        uint32_t mask = 0;
 #pragma unroll
-      for (int k = 0; k < 8; k++) mask |= (v[k] <= st.thr) ? (1u << (8 * (k >> 1) + 2 * sub + (k & 1))) : 0u;
-      mask |= __shfl_xor_sync(qmask, mask, 1);
-      mask |= __shfl_xor_sync(qmask, mask, 2);
-      if (sub == 0) {
-        if (st.n_staged == kCandSlots) {         // compact against the (tighter) current threshold
-          int keep = 0;
-          for (int k = 0; k < kCandSlots; k++) {
-            const float sv = sh.cand_val[k * BM + etid];
-            if (sv <= st.thr) {
-              sh.cand_val[keep * BM + etid] = sv;
-              sh.cand_col[keep * BM + etid] = sh.cand_col[k * BM + etid];
-              sh.cand_mask[keep * BM + etid] = sh.cand_mask[k * BM + etid];
-              keep++;
-            }
-          }
-          st.n_staged = keep;
-        }
-        if (st.n_staged < kCandSlots) {
-          sh.cand_val[st.n_staged * BM + etid] = mn;
-          sh.cand_col[st.n_staged * BM + etid] = cbase;
-          sh.cand_mask[st.n_staged * BM + etid] = mask;
-          st.n_staged++;
-        } else {                                 // staging full of live chunks: emit directly
-          const int pos = atomicAdd(args.cand_cnt + st.row, 1);
-          if (pos < args.cap) {
-            args.cand_idx[(st.row * args.cap + pos) * 2] = cbase;
-            args.cand_idx[(st.row * args.cap + pos) * 2 + 1] = (int)mask;
-          }
-        }
+        for (int k = 0; k < 8; k++) mask |= (v[k] <= st.thr) ? (1u << (8 * (k >> 1) + 2 * sub + (k & 1))) : 0u;
+        mask |= __shfl_xor_sync(qmask, mask, 1);
+        mask |= __shfl_xor_sync(qmask, mask, 2);
+        if (sub == 0) stage_chunk(args, sh, etid, st.n_staged, st.row, cbase, mask, mn, st.thr);
       }
+      return;
+    }
+    if (event && mn < st.best) {
+      st.best = mn;
+      st.s_ref = fminf(st.s_ref, fmaxf(st.best + st.nx, 0.f));
+      st.thr = nn_threshold(st.s_ref, st.nx, st.e2, st.g);
+    }
+    // exact per-column mask of the chunk: the re-rank then touches only rows inside the window.  Built by the whole
+    // warp (used only on an event): shuffles inside the divergent event branch make ptxas serialise the wgmma.
+    uint32_t mask = 0;
+#pragma unroll
+    for (int k = 0; k < 8; k++) mask |= (v[k] <= st.thr) ? (1u << (8 * (k >> 1) + 2 * sub + (k & 1))) : 0u;
+    mask |= __shfl_xor_sync(0xffffffffu, mask, 1);
+    mask |= __shfl_xor_sync(0xffffffffu, mask, 2);
+    if (event) {
+      ev |= 1 << c;
+      if (sub == 0) rec[c] = EvRecord{cbase, mask, mn, st.thr};
     }
   } else if (MODE == MODE_LSE) {
     constexpr float kL2e = 1.4426950408889634f;
@@ -344,8 +405,15 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   const uint32_t a_full = bar0 + 8u * (2 * kStages), a_empty = bar0 + 8u * (2 * kStages + 1);
   auto sched_full = [&](int s) { return bar0 + 8u * (2 * kStages + 2 + s); };
   auto sched_empty = [&](int s) { return bar0 + 8u * (2 * kStages + 4 + s); };
-  volatile int* sched_ring = reinterpret_cast<volatile int*>(smem + kRingBytes + 8 * (2 * kStages + 6));
-  static_assert(8 * (2 * kStages + 6) + 8 <= kBarBytes, "barrier block");
+  auto ev_full = [&](int b) { return bar0 + 8u * (2 * kStages + 6 + b); };
+  auto ev_empty = [&](int b) { return bar0 + 8u * (2 * kStages + 8 + b); };
+  volatile int* sched_ring = reinterpret_cast<volatile int*>(smem + kRingBytes + 8 * (2 * kStages + 10));
+  static_assert(8 * (2 * kStages + 10) + 8 <= kBarBytes, "barrier block");
+  EpiShared sh;   // MODE_NN candidate staging: drain warps (resident variant) / consumers (streaming variant)
+  sh.cand_val = reinterpret_cast<float*>(smem + kRingBytes + kBarBytes);
+  sh.cand_col = reinterpret_cast<int*>(sh.cand_val + kCandSlots * BM);
+  sh.cand_mask = reinterpret_cast<uint32_t*>(sh.cand_col + kCandSlots * BM);
+  EvBuf* evbuf = reinterpret_cast<EvBuf*>(smem + kRingBytes + kBarBytes + kCandBytes);
 
   // warp index through a shuffle: provably warp-uniform, so the compiler keeps the consumers' wgmma asynchronous
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
@@ -365,6 +433,7 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     mbar_init(a_full, 1);
     mbar_init(a_empty, kConsumerWarps);
     for (int s = 0; s < 2; s++) { mbar_init(sched_full(s), 1); mbar_init(sched_empty(s), kConsumerWarps); }
+    for (int b = 0; b < 2; b++) { mbar_init(ev_full(b), kConsumerWarps); mbar_init(ev_empty(b), kDrainWarps); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -432,19 +501,54 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       }
     }
     __syncwarp();
-  } else if (warp >= 4) {
+  } else if (warp < 4) {
+    // ================= MODE_NN drain (resident variant): stage the consumers' events =================
+    // Thread dt owns local rows dt and dt + 96: their staging slots and counts.  Per row, events arrive in column
+    // order.  An event is staged unless it is dead against the tighter of the record's thr and the row's thr after
+    // its tile; with the slots full they are compacted against that threshold, and a chunk that still finds them
+    // full of live chunks goes straight to the row's list.  The last tile of an item flushes the slots that
+    // survive the row's final thr (read by the consumers after the item, from the shared running minimum).
+    if (MODE == MODE_NN && RESA) {
+      const int dt = threadIdx.x - 32;
+      int n_staged[2] = {0, 0};
+      for (int qt = 0;; qt++) {
+        const int b = qt & 1;
+        mbar_wait(ev_full(b), (uint32_t)(qt >> 1) & 1u);
+        const EvBuf& e = evbuf[b];
+        const int flags = e.flags;
+        if (flags & kEvStop) break;
+        const bool stamp = args.timeline && blockIdx.x == 0 && dt == 0 && qt < args.timeline_tiles;
+        if (stamp) args.timeline[(int64_t)qt * 16 + 11] = clock64();
+#pragma unroll
+        for (int j = 0; j < 2; j++) {
+          const int r = dt + 32 * kDrainWarps * j;
+          if (r >= BM) continue;
+          const EvRow er = e.row[r];
+          const int64_t row = (int64_t)e.q_row0 + r;
+          for (int c = 0; c < kEvSlots; c++) {
+            if (!((er.ev >> c) & 1)) continue;
+            const EvRecord rc = e.rec[r * kEvSlots + c];
+            const float thr = fminf(rc.thr, er.thr);
+            if (rc.mn <= thr) stage_chunk(args, sh, r, n_staged[j], row, rc.col, rc.mask, rc.mn, thr);
+          }
+          if (flags & kEvLast) {
+            flush_row(args, sh, r, n_staged[j], row, er.thr);
+            n_staged[j] = 0;
+          }
+        }
+        if (stamp) args.timeline[(int64_t)qt * 16 + 12] = clock64();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(ev_empty(b));
+      }
+    }
+  } else {
     // ================= consumers: wgmma + register epilogue =================
     const int cw = warp - 4;                    // consumer warp 0..7
     const int g = cw >> 2;                        // consumer warpgroup: query rows [64 g, 64 g + 64)
     const int sub = lane & 3;
-    const unsigned qmask = 0xFu << (lane & 28);   // the lanes of this quad
     const int lead = lane & 28;                   // the quad's first lane
     // accumulator register i holds row 16 (warp % 4) + lane / 4 + 8 ((i / 2) % 2), column 8 (i / 4) + 2 (lane % 4) + i % 2
     const int row_h0 = g * 64 + (cw & 3) * 16 + (lane >> 2);
-    EpiShared sh;
-    sh.cand_val = reinterpret_cast<float*>(smem + kRingBytes + kBarBytes);
-    sh.cand_col = reinterpret_cast<int*>(sh.cand_val + kCandSlots * BM);
-    sh.cand_mask = reinterpret_cast<uint32_t*>(sh.cand_col + kCandSlots * BM);
     const float kInf = __int_as_float(0x7f800000);
     float acc[64];
     int stage = 0, rel_stage = 0;  // next stage to consume / to release
@@ -452,13 +556,22 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     int a_row0 = -1;
     bool first_item = true;
     int tl_tile0 = 0;           // timeline index of the item's first tile
+    int qt = 0;                 // MODE_NN: tiles handed to the drain so far (mailbox qt & 1)
     for (int k = 0;; k++) {
       const int slot = k & 1;
       mbar_wait(sched_full(slot), (uint32_t)(k >> 1) & 1u);
       const int w = sched_ring[slot];
       __syncwarp();
       if (lane == 0) mbar_arrive(sched_empty(slot));
-      if (w < 0) break;
+      if (w < 0) {
+        if (MODE == MODE_NN && RESA) {   // release the drain warps
+          mbar_wait(ev_empty(qt & 1), ((uint32_t)(qt >> 1) & 1u) ^ 1u);
+          if (cw == 0 && lane == 0) evbuf[qt & 1].flags = kEvStop;
+          __syncwarp();
+          if (lane == 0) mbar_arrive(ev_full(qt & 1));
+        }
+        break;
+      }
       const tip_work_item it = args.items[w];
       const int ntiles = (it.col1 - it.col0 + BN - 1) / BN;
       if (ntiles <= 0) continue;
@@ -516,31 +629,29 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       args.timeline[(int64_t)(tl_tile0 + (t)) * 16 + (slot)] = clock64();                                 \
   } while (0)
 
-      // Resident query tile: issue the MMAs of tile t into acc, one commit group per K chunk, all of them in flight
-      // before the first wait; retire_tile waits and releases their stages.
-      auto issue_tile = [&](int t) {
+      // Resident query tile: issue the MMAs of tile t into `a`, one commit group for the whole tile.
+      auto issue_tile = [&](float (&a)[64], int t) {
         TLT(t, 0);
+        acc_fence(a);
         for (int c = 0; c < nchunks; c++) {
           mbar_wait(full_bar(stage), phase);
           const uint32_t a_addr = base + (uint32_t)c * kABytes + (uint32_t)g * 64 * 128;
           const uint32_t b_addr = b_ring + (uint32_t)stage * kBBytes;
           const uint64_t adesc = smem_desc(a_addr), bdesc = smem_desc(b_addr);
           const int nm = min(4, k16 - 4 * c);
-          acc_fence(acc);
           wgmma_fence();
-          wgmma_m64n128k16<F16>(acc, adesc, bdesc, c > 0 ? 1u : 0u);
-          for (int kk = 1; kk < nm; kk++) wgmma_m64n128k16<F16>(acc, adesc + 2u * kk, bdesc + 2u * kk, 1u);
-          wgmma_commit();
-          acc_fence(acc);
+          wgmma_m64n128k16<F16>(a, adesc, bdesc, c > 0 ? 1u : 0u);
+          for (int kk = 1; kk < nm; kk++) wgmma_m64n128k16<F16>(a, adesc + 2u * kk, bdesc + 2u * kk, 1u);
           if (++stage == kStages) { stage = 0; phase ^= 1u; }
         }
+        wgmma_commit();
+        acc_fence(a);
       };
-      // Wait for every MMA in flight (the tile in acc), then release the stages not released yet.
-      auto retire_tile = [&](int t, int n_release) {
-        wgmma_wait_all();
-        acc_fence(acc);
+      // Tile t in `a` has retired (the caller waited): release its stages.
+      auto retire_tile = [&](float (&a)[64], int t) {
+        acc_fence(a);
         __syncwarp();
-        for (int c = 0; c < n_release; c++) {
+        for (int c = 0; c < nchunks; c++) {
           if (lane == 0) mbar_arrive(empty_bar(rel_stage));
           if (++rel_stage == kStages) rel_stage = 0;
         }
@@ -554,15 +665,20 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
           if (MODE == MODE_NN && st[h].valid_row && sub == 0) sb[h] = ld_volatile_u32(args.row_min_bits + st[h].row);
         }
       };
-      auto epilogue = [&](int t, const uint32_t (&sb)[2]) {
+      auto epilogue = [&](float (&a)[64], int t, const uint32_t (&sb)[2]) {
         const int col_base = it.col0 + t * BN;
         const bool partial = col_base + BN > it.col1;
+        const bool last = t == ntiles - 1;
+        EvBuf* eb = evbuf + (qt & 1);
+        int ev[2] = {0, 0};
+        // a free mailbox (convergent: the drain released it two tiles ago)
+        if (MODE == MODE_NN) mbar_wait(ev_empty(qt & 1), ((uint32_t)(qt >> 1) & 1u) ^ 1u);
         if (MODE == MODE_DUMP) {
           if (dump_item && t < 2) {     // the first 128 rows x 256 columns of the first item
 #pragma unroll
             for (int i = 0; i < 64; i++) {
               const int col = t * BN + 8 * (i >> 2) + 2 * sub + (i & 1);
-              args.dump[(int64_t)(row_h0 + 8 * ((i >> 1) & 1)) * 256 + col] = acc[i];
+              args.dump[(int64_t)(row_h0 + 8 * ((i >> 1) & 1)) * 256 + col] = a[i];
             }
           }
         } else {
@@ -574,8 +690,8 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             float m[2] = {kInf, kInf};
 #pragma unroll
             for (int i = 0; i < 64; i += 4) {
-              m[0] = fminf(m[0], fminf(acc[i], acc[i + 1]));
-              m[1] = fminf(m[1], fminf(acc[i + 2], acc[i + 3]));
+              m[0] = fminf(m[0], fminf(a[i], a[i + 1]));
+              m[1] = fminf(m[1], fminf(a[i + 2], a[i + 3]));
             }
             any = __any_sync(0xffffffffu, (st[0].valid_row && m[0] <= st[0].thr) || (st[1].valid_row && m[1] <= st[1].thr));
           }
@@ -587,10 +703,11 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
                 float v[8];
 #pragma unroll
                 for (int jj = 0; jj < 4; jj++) {
-                  v[2 * jj] = acc[4 * (4 * c + jj) + 2 * h];
-                  v[2 * jj + 1] = acc[4 * (4 * c + jj) + 2 * h + 1];
+                  v[2 * jj] = a[4 * (4 * c + jj) + 2 * h];
+                  v[2 * jj + 1] = a[4 * (4 * c + jj) + 2 * h + 1];
                 }
-                epi_chunk<MODE, EXCL>(args, st[h], sh, v, col_base + 32 * c, sub, qmask, partial, row_h0 + 8 * h);
+                epi_chunk<MODE, EXCL, RESA>(args, st[h], sh, eb->rec + (row_h0 + 8 * h) * kEvSlots, ev[h], v,
+                                            col_base + 32 * c, c, sub, partial, row_h0 + 8 * h);
               }
             }
           }
@@ -608,7 +725,24 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
               s.s_ref = seen;
               s.thr = nn_threshold(s.s_ref, s.nx, s.e2, s.g);
             }
+            if (last && sub == 0) {
+              // other CTAs have been scanning other columns of this query meanwhile: the drain flushes only the
+              // chunks that survive the best bound known by now (the quad's other lanes are done with this row)
+              const float now = __uint_as_float(ld_volatile_u32(args.row_min_bits + s.row));
+              if (now < s.s_ref) {
+                s.s_ref = now;
+                s.thr = nn_threshold(s.s_ref, s.nx, s.e2, s.g);
+              }
+            }
           }
+          // hand the tile's events to the drain: per row its thr after the tile and the chunks with an event
+#pragma unroll
+          for (int h = 0; h < 2; h++)
+            if (sub == 0) eb->row[row_h0 + 8 * h] = EvRow{st[h].thr, ev[h]};
+          if (cw == 0 && lane == 0) { eb->q_row0 = it.q_row0; eb->flags = last ? kEvLast : 0; }
+          __syncwarp();
+          if (lane == 0) mbar_arrive(ev_full(qt & 1));
+          qt++;
         }
         TLT(t, 7);
       };
@@ -616,10 +750,11 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       if (RESA) {
         for (int t = 0; t < ntiles; t++) {
           uint32_t sb[2];
-          issue_tile(t);
+          issue_tile(acc, t);
           load_seen(sb);
-          retire_tile(t, nchunks);
-          epilogue(t, sb);
+          wgmma_wait_all();
+          retire_tile(acc, t);
+          epilogue(acc, t, sb);
         }
       } else {
         // streaming (wide rows, many chunks per tile): the MMA loop dominates; each chunk is retired before the next
@@ -670,7 +805,9 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
                   v[2 * jj] = acc[4 * (4 * c + jj) + 2 * h];
                   v[2 * jj + 1] = acc[4 * (4 * c + jj) + 2 * h + 1];
                 }
-                epi_chunk<MODE, EXCL>(args, st[h], sh, v, col_base + 32 * c, sub, qmask, partial, row_h0 + 8 * h);
+                int ev = 0;
+                epi_chunk<MODE, EXCL, RESA>(args, st[h], sh, nullptr, ev, v, col_base + 32 * c, c, sub, partial,
+                                            row_h0 + 8 * h);
               }
             }
           }
@@ -698,8 +835,7 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       for (int h = 0; h < 2; h++) {
         EpiState& s = st[h];
         if (!s.valid_row || sub != 0) continue;
-        const int etid = row_h0 + 8 * h;
-        if (MODE == MODE_NN) {
+        if (MODE == MODE_NN && !RESA) {
           // other CTAs have been scanning other columns of this query meanwhile: only flush the groups that
           // survive the best bound known by now
           const float seen = __uint_as_float(ld_volatile_u32(args.row_min_bits + s.row));
@@ -707,15 +843,7 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             s.s_ref = seen;
             s.thr = nn_threshold(s.s_ref, s.nx, s.e2, s.g);
           }
-          for (int q = 0; q < s.n_staged; q++) {
-            if (sh.cand_val[q * BM + etid] <= s.thr) {
-              const int pos = atomicAdd(args.cand_cnt + s.row, 1);
-              if (pos < args.cap) {
-                args.cand_idx[(s.row * args.cap + pos) * 2] = sh.cand_col[q * BM + etid];
-                args.cand_idx[(s.row * args.cap + pos) * 2 + 1] = (int)sh.cand_mask[q * BM + etid];
-              }
-            }
-          }
+          flush_row(args, sh, row_h0 + 8 * h, s.n_staged, s.row, s.thr);
         } else if (MODE == MODE_LSE) {
           args.part_max[(int64_t)it.slot * args.m + s.row] = s.run_max;
           args.part_sum[(int64_t)it.slot * args.m + s.row] = s.run_sum;

@@ -6,7 +6,9 @@ Runs C2's stage-1 (same-class columns) and stage-2 (other-class columns) searche
 `tip_debug_timeline` on and turns the stamps of block 0 into per-tile phases, in SM clocks:
   mma      consumer: first MMA issue of the tile (slot 0) -> its MMAs retired (slot 1), including the
            waits for the tile's chunks to land
-  epilogue consumer: MMAs retired (slot 1) -> reduction done (slot 7)
+  epilogue consumer: MMAs retired (slot 1) -> reduction done and events handed to the drain (slot 7)
+  drain    drain warps: the tile's events received (slot 11) -> staged / emitted (slot 12); a build without
+           drain warps reports null
   period   consumer: tile start -> next tile start (slot 0 to slot 0)
   lead     producer ahead of the consumers: producer starts loading the tile (slot 8) -> consumer starts
            issuing it (slot 0); large means the ring is full and the consumers are the limit
@@ -65,6 +67,9 @@ def main():
         t = t[(t[:, 0] > 0) & (t[:, 1] > 0) & (t[:, 7] > 0) & (t[:, 8] > 0) & (t[:, 10] > 0)]
         ph = {"mma": t[:, 1] - t[:, 0], "epilogue": t[:, 7] - t[:, 1], "period": np.diff(t[:, 0]),
               "lead": t[:, 0] - t[:, 8], "load": t[:, 10] - t[:, 8]}
+        d = buf.cpu().numpy()
+        d = d[(d[:, 11] > 0) & (d[:, 12] > 0)]
+        ph["drain"] = d[:, 12] - d[:, 11]
         rec = {"tiles": int(len(t)), "search_ms": ev0.elapsed_time(ev1)}
         for k, v in ph.items():
             rec[k] = {"p50": float(np.percentile(v, 50)), "p90": float(np.percentile(v, 90))} if len(v) else None
