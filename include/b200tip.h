@@ -40,6 +40,9 @@
  *   tip_gmm_scatter     sklearn _estimate_gaussian_covariances_full: (resp_k * diff.T) @ diff / nk + reg_covar I
  *   tip_cov_location    src/core/surprise.py:385-386 EmpiricalCovariance().fit: location_ = X.mean(0) and
  *                       np.cov's float64 centring mean (the scatter reuses tip_gmm_scatter)
+ *   tip_col_var         src/core/surprise.py:421,433 LSA's column selection: np.var(x, axis=0), bit for bit
+ *   tip_whiten_dmma     scipy==1.4.1 gaussian_kernel_estimate: dataset . cholesky(inv_cov) for the training rows
+ *                       of LSA's device fit, fp64 DMMA (the covariance reuses tip_gmm_scatter)
  */
 #ifndef B200TIP_H
 #define B200TIP_H
@@ -485,6 +488,20 @@ int tip_gmm_scatter(const void* x, int dtype, int64_t n, int64_t d, const double
  * The scatter of the fit is tip_gmm_scatter with k = 1, unit weights, means = mean and nk = {n}. */
 int tip_cov_location(const void* x, int dtype, int64_t n, int64_t d, void* location, double* mean,
                      int32_t* flags, void* stream);
+
+/* ---- LSA's KDE fit (StableGaussianKDE on the device) ------------------------------------------------------
+ * tip_col_var: x n x d (TIP_F32/TIP_F64), 1 <= n < 2^31, 1 <= d <= 65536.  var[d] (x's dtype) = np.var(x, axis=0)
+ * bit for bit as NumPy 2.3's _methods._var computes it: the mean of tip_cov_location, then (x - mean) in x's
+ * dtype, squared as a separate rounding, reduced like the mean (sequential over the rows for d >= 2, pairwise for
+ * d == 1) and divided by n in double, rounded once.  mean[d] and *flags as tip_cov_location.
+ * tip_whiten_dmma: out[m x d_out] (fp32) = (x[:, cols] - mu) . w, x: m x d_in (TIP_F32/TIP_F64), cols[d_out]
+ * (NULL = all, then d_in == d_out), mu: d_out doubles, w: d_out x d_out doubles row-major, LOWER triangular
+ * (entries above the diagonal are never read), 1 <= d_out <= 65536.  Accumulated in float64 on the fp64 tensor
+ * cores, rounded once to fp32.  Deterministic (fixed order, no atomics). */
+int tip_col_var(const void* x, int dtype, int64_t n, int64_t d, void* var, double* mean, int32_t* flags,
+                void* stream);
+int tip_whiten_dmma(const void* x, int dtype, int64_t m, int64_t d_in, const int32_t* cols, int64_t d_out,
+                    const double* mu, const double* w_lower, float* out, void* stream);
 
 /* ---- bring-up / validation: plain accumulator dump ------------------------------------
  * out[256*256] (fp32, row-major, leading dimension 256) = tail-augmented dot products of q rows

@@ -100,6 +100,8 @@ _SIGNATURES = {
     "tip_gmm_moments": (C.c_int, [_vp, C.c_int, _i64, _i64, _vp, _i32, _vp, _vp, _vp, _vp, _vp]),
     "tip_gmm_scatter": (C.c_int, [_vp, C.c_int, _i64, _i64, _vp, _vp, _i32, _vp, C.c_double, _i32, _vp, _vp, _vp]),
     "tip_cov_location": (C.c_int, [_vp, C.c_int, _i64, _i64, _vp, _vp, _vp, _vp]),
+    "tip_col_var": (C.c_int, [_vp, C.c_int, _i64, _i64, _vp, _vp, _vp, _vp]),
+    "tip_whiten_dmma": (C.c_int, [_vp, C.c_int, _i64, _i64, _vp, _i64, _vp, _vp, _vp, _vp]),
 }
 
 _lock = threading.Lock()

@@ -85,26 +85,82 @@ class StableGaussianKDE:
         self.prepare_failed = False
         return covariance
 
-    # -- device state ----------------------------------------------------------------------
-    def _upload(self):
+    @classmethod
+    def from_device(cls, x, cols: Optional[np.ndarray] = None, mean=None, timing: Optional[dict] = None
+                    ) -> "StableGaussianKDE":
+        """StableGaussianKDE(x[:, cols].T) fitted on the GPU (engine.kde_fit, float64): x is an [n, D] float32 /
+        float64 device matrix, cols the kept source columns (None: all of them), mean x's float64 column mean
+        (engine.col_var's, optional).  Same attributes and errors as the host fit; dataset, covariance, inv_cov,
+        whitening, _data_covariance, _data_inv_cov and mean are held on the device and copied to the host on first
+        access.  The training operand is the fit's own fp32 (x[:, cols] - mean) @ W, which never leaves the GPU."""
         import torch
 
         from .. import engine as E
 
+        n, width = int(x.shape[0]), int(x.shape[1])
+        d = width if cols is None else len(cols)
+        if not n * d > 1:
+            raise ValueError("`dataset` input should have multiple elements.")
+        self = cls.__new__(cls)
+        self.d, self.n = d, n
+        self.weights = np.ones(self.n) / self.n
+        self.neff = 1.0 / np.sum(self.weights ** 2)
+        self.source_columns = None if cols is None else np.asarray(cols, dtype=np.int32)
+        self._engine, self._comm = None, None
+        fit = E.kde_fit(x, cols, mean, timing)
+        self.factor = fit["factor"]
+        self.prepare_failed = fit["prepare_failed"]
+        rows = fit["rows"]
+        f2 = self.factor ** 2
+        self._lazy = {"dataset": lambda: rows.t().to(torch.float64), "mean": lambda: fit["mean"]}
+        if "covariance" not in fit:                  # failed fit: the host keeps no inverse either
+            self._data_inv_cov = None
+            return self
+        self._lazy.update({"_data_covariance": lambda: fit["covariance"], "_data_inv_cov": lambda: fit["inv"],
+                           "covariance": lambda: fit["covariance"] * f2, "inv_cov": lambda: fit["inv"] / f2,
+                           "whitening": lambda: fit["whitening"]})
+        self.log_det = fit["log_det"]
+        self._norm_factor = fit["norm_factor"]
+        self._attach(fit["diag_w"], fit["p"], fit["whitening"].to(torch.float32), fit["mean"])
+        return self
+
+    def __getattr__(self, name):
+        """device-held attributes of a from_device fit, copied to the host on first access"""
+        lazy = self.__dict__.get("_lazy")
+        if lazy is None or name not in lazy:
+            raise AttributeError(f"{type(self).__name__!r} object has no attribute {name!r}")
+        value = lazy.pop(name)().cpu().numpy()
+        setattr(self, name, value)
+        return value
+
+    # -- device state ----------------------------------------------------------------------
+    def _upload(self):
+        import torch
+
         self.whitening = np.linalg.cholesky(self.inv_cov)                 # scipy 1.4.1: cholesky(precision)
         self.mean = self.dataset.mean(axis=1)
-        norm = math.pow(2 * math.pi, -self.d / 2.0)
-        for i in range(self.d):
-            norm *= self.whitening[i, i]
-        self.norm = norm
-        self.log_norm = -self.d / 2.0 * math.log(2 * math.pi) + float(np.sum(np.log(np.diag(self.whitening))))
         # squared distances are translation invariant: centre before whitening so the split-bf16
         # operands carry the spread, not the offset, of the traces
         p = (self.dataset.T - self.mean) @ self.whitening
+        self._attach(np.diag(self.whitening), p, torch.from_numpy(self.whitening.astype(np.float32)),
+                     torch.from_numpy(self.mean))
+
+    def _attach(self, diag_w: np.ndarray, p, w32, mu):
+        """norm / log_norm from the whitening factor's diagonal, the KDE engine over the training operand p, and the
+        query whitening's device operands (w32 fp32 [d, d], mu float64 [d])."""
+        import torch
+
+        from .. import engine as E
+
+        norm = math.pow(2 * math.pi, -self.d / 2.0)
+        for i in range(self.d):
+            norm *= diag_w[i]
+        self.norm = norm
+        self.log_norm = -self.d / 2.0 * math.log(2 * math.pi) + float(np.sum(np.log(diag_w)))
         self._engine = E.KdeEngine(p, self._comm)
         dev = self._engine.dev
-        self._w_dev = torch.from_numpy(self.whitening.astype(np.float32)).to(dev)
-        self._mu_dev = torch.from_numpy(self.mean).to(dev)
+        self._w_dev = w32.to(dev)
+        self._mu_dev = mu.to(dev)
         self._cols_dev = None if self.source_columns is None else torch.from_numpy(self.source_columns).to(dev)
 
     # -- score -----------------------------------------------------------------------------

@@ -116,6 +116,14 @@ def _cov_backend(backend: Optional[str]) -> str:
     return backend
 
 
+def _kde_backend(backend: Optional[str]) -> str:
+    """backend=None: the B200TIP_KDE environment variable, default "host"."""
+    backend = backend if backend is not None else os.environ.get("B200TIP_KDE", "host")
+    if backend not in ("host", "device"):
+        raise ValueError(f"backend must be 'host' or 'device', got {backend!r}")
+    return backend
+
+
 def _trace_matrix(activations):
     """[N, D] traces: the device matrix for torch CUDA traces, else the reference's host flattening."""
     from .. import engine as E
@@ -237,6 +245,19 @@ class MultiModalSA(SA):
 
     @staticmethod
     def build(activations, predictions, discriminator: Discriminator, sa_constructor) -> "MultiModalSA":
+        """CUDA traces (one tensor or a list of hook layers) are split by modal on the device, and the constructors
+        receive CUDA tensors; NumPy traces are split on the host, as the reference does."""
+        from .. import engine as E
+
+        x = E.device_matrix(activations)
+        if x is not None:
+            preds = _flatten_predictions(E.host_array(predictions))
+            modal = E.host_array(discriminator(x, preds))
+            fitted: Dict[int, SA] = {}
+            for mid in np.unique(modal):
+                rows = np.flatnonzero(modal == mid)
+                fitted[mid] = sa_constructor(_take_rows(x, rows), None if preds is None else preds[rows])
+            return MultiModalSA(discriminator=discriminator, modal_sa=fitted)
         acts = _flatten_layers(activations)
         preds = _flatten_predictions(predictions)
         modal = discriminator(acts, preds)
@@ -451,14 +472,37 @@ class LSA(SA):
     """Likelihood-based surprise adequacy (surprise.py:396-495).
 
     fit: highest-variance column selection (:417-434) and the float64 KDE fit of
-    `StableGaussianKDE` on the host; score: whitening + fused Gaussian-KDE log-sum-exp on the
-    GPU, then `-np.log(density)` (:494-495; +inf where the float64 density underflows to 0)."""
+    `StableGaussianKDE`; score: whitening + fused Gaussian-KDE log-sum-exp on the
+    GPU, then `-np.log(density)` (:494-495; +inf where the float64 density underflows to 0).
+    backend="host" (default, or B200TIP_KDE unset): the fit is the reference's host NumPy.  backend="device": np.var
+    bit for bit (tip_col_var), the covariance, its factorisations and the training-row whitening in float64 on the
+    GPU (StableGaussianKDE.from_device); the column selection stays the reference's host expression, run on the
+    downloaded variances.  Traces may be torch CUDA tensors under either backend (the host backend downloads them);
+    bf16 / fp16 CUDA traces are widened to float32."""
 
     def __init__(self, activations: Activations, var_threshold: Optional[float] = None,
-                 max_features: Optional[Union[int, float]] = 300, *, comm=None):
+                 max_features: Optional[Union[int, float]] = 300, *, comm=None, backend: Optional[str] = None):
         super().__init__()
+        import torch
+
+        from .. import engine as E
+
         self._comm = comm         # additive: N_train-sharded KDE evaluation (engine.TrainShardComm)
-        activations = _flatten_layers(activations)
+        self.backend = _kde_backend(backend)
+        if self.backend == "device" and comm is not None and comm.world > 1:
+            raise NotImplementedError("the device KDE fit is not sharded over N_train; use backend='host' with comm")
+        dev = E.device_matrix(activations)
+        if dev is not None and dev.dtype not in (torch.float32, torch.float64):
+            dev = dev.float()
+        if self.backend == "device":
+            E.require_cuda()
+            activations = _device_rows(activations if dev is None else dev)
+            var_dev, self._mean, _ = E.col_var(activations)
+            var = var_dev.cpu().numpy()
+            variances = lambda: var       # noqa: E731  (identical bits to np.var(activations, axis=0))
+        else:
+            activations = dev.cpu().numpy() if dev is not None else _flatten_layers(activations)
+            variances = lambda: np.var(activations, axis=0)       # noqa: E731
         self._source_width = int(activations.shape[1])
         assert var_threshold is None or max_features is None, (
             "Both var_threshold and max_features cannot be specified at the same time."
@@ -466,14 +510,28 @@ class LSA(SA):
             "with the highest variance.")
         self.removed_neurons: List[int]
         if var_threshold is not None and var_threshold > 0:
-            self.removed_neurons = np.where(np.var(activations, axis=0) < var_threshold)[0]
+            self.removed_neurons = np.where(variances() < var_threshold)[0]
         if max_features is not None:
             width = activations.shape[1]
             keep = min(max_features * width, width) if max_features < 1 else min(max_features, width)
-            self.removed_neurons = [int(c) for c in np.argsort(np.var(activations, axis=0))[:-keep]]
+            self.removed_neurons = [int(c) for c in np.argsort(variances())[:-keep]]
         self.kde = self._create_gaussian_kde(activations)
 
-    def _create_gaussian_kde(self, activations: np.ndarray):
+    def _create_gaussian_kde(self, activations):
+        if self.backend == "device":
+            kept = np.delete(np.arange(activations.shape[1]), self.removed_neurons)
+            if kept.size == 0:
+                warnings.warn("All activation traces were removed (variance filter); this LSA instance "
+                              "will always report density 0", UserWarning)
+                self.kde = None
+                return None
+            try:
+                return StableGaussianKDE.from_device(activations, kept if len(self.removed_neurons) > 0 else None,
+                                                     self._mean)
+            except (np.linalg.LinAlgError, ValueError) as e:
+                # the device fit raises neither of the two messages the reference retries on (see below)
+                warnings.warn("Problem regarding KDE fitting", UserWarning)
+                raise e
         cleaned = self._remove_unused_columns(activations)
         if cleaned.shape[1] == 0:
             warnings.warn("All activation traces were removed (variance filter); this LSA instance "

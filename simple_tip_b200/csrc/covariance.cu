@@ -14,6 +14,11 @@
 // The division is done in double and rounded once to the input dtype, which is the correctly rounded quotient for
 // float32 as well (NumPy divides float32 by an intp in double and casts back).  Non-finite inputs set flags bits
 // (1: NaN, 2: +-inf) so that the fit can raise sklearn's error instead of returning NaN.
+//
+// tip_col_var (LSA's column selection, np.var(x, axis=0)) runs the same kernels with a second pass over the rows:
+// NumPy 2.3's _methods._var subtracts the input-dtype mean above (arr - arrmean, in x's dtype), squares with
+// multiply(x, x) as a rounding of its own (no FMA), reduces that with the same add.reduce (sequential for d >= 2,
+// pairwise for d == 1) and divides by the intp count the same way.
 #include "common.cuh"
 
 namespace tip {
@@ -33,7 +38,7 @@ __device__ __forceinline__ T cov_div(T s, int64_t n) {
 template <typename T>
 __global__ void __launch_bounds__(kCovThreads) cov_location_kernel(const T* __restrict__ x, int64_t n, int64_t d,
                                                                    T* __restrict__ loc, double* __restrict__ mean,
-                                                                   int32_t* __restrict__ flags) {
+                                                                   T* __restrict__ var, int32_t* __restrict__ flags) {
   using R = Rn<T>;
   const int64_t c = (int64_t)blockIdx.x * kCovThreads + threadIdx.x;
   if (c >= d) return;
@@ -58,37 +63,56 @@ __global__ void __launch_bounds__(kCovThreads) cov_location_kernel(const T* __re
     s64 = __dadd_rn(s64, (double)v);
     flag |= cov_flag((double)v);
   }
-  loc[c] = cov_div<T>(s, n);
+  const T m = cov_div<T>(s, n);
+  if (loc) loc[c] = m;
   mean[c] = __ddiv_rn(s64, (double)n);
   if (flag) atomicOr(flags, flag);      // an integer flag: the result does not depend on the order
+  if (!var) return;
+  // np.var's second pass: arr - arrmean, then multiply(x, x) as its own rounding, summed in row order
+  T s2 = (T)0;
+  for (r = 0; r + kCovUnroll <= n; r += kCovUnroll) {
+    T v[kCovUnroll];
+#pragma unroll
+    for (int u = 0; u < kCovUnroll; u++) v[u] = x[(r + u) * d + c];
+#pragma unroll
+    for (int u = 0; u < kCovUnroll; u++) {
+      const T e = R::sub(v[u], m);
+      s2 = R::add(s2, R::mul(e, e));
+    }
+  }
+  for (; r < n; r++) {
+    const T e = R::sub(x[r * d + c], m);
+    s2 = R::add(s2, R::mul(e, e));
+  }
+  var[c] = cov_div<T>(s2, n);
 }
 
-// one leaf (n <= 128) of NumPy's pairwise sum, accumulated in A
-template <typename A, typename T>
-__device__ A cov_leaf(const T* __restrict__ x, int n) {
+// one leaf [o, o + n) (n <= 128) of NumPy's pairwise sum of term(i), accumulated in A
+template <typename A, typename F>
+__device__ A cov_leaf(const F& term, int o, int n) {
   using R = Rn<A>;
   if (n < 8) {
     A res = (A)0;
-    for (int i = 0; i < n; i++) res = R::add(res, (A)x[i]);
+    for (int i = 0; i < n; i++) res = R::add(res, term(o + i));
     return res;
   }
   A r[8];
 #pragma unroll
-  for (int j = 0; j < 8; j++) r[j] = (A)x[j];
+  for (int j = 0; j < 8; j++) r[j] = term(o + j);
   int i = 8;
   const int lim = n - (n % 8);
   for (; i < lim; i += 8)
 #pragma unroll
-    for (int j = 0; j < 8; j++) r[j] = R::add(r[j], (A)x[i + j]);
+    for (int j = 0; j < 8; j++) r[j] = R::add(r[j], term(o + i + j));
   A res = R::add(R::add(R::add(r[0], r[1]), R::add(r[2], r[3])), R::add(R::add(r[4], r[5]), R::add(r[6], r[7])));
-  for (; i < n; i++) res = R::add(res, (A)x[i]);
+  for (; i < n; i++) res = R::add(res, term(o + i));
   return res;
 }
 
-// NumPy's pairwise sum of x[0, n) accumulated in A, with an explicit stack (depth <= 32 for n < 2^31)
-template <typename A, typename T>
-__device__ A cov_pairwise(const T* __restrict__ x, int n) {
-  if (n <= 128) return cov_leaf<A, T>(x, n);
+// NumPy's pairwise sum of term(0 .. n-1) accumulated in A, with an explicit stack (depth <= 32 for n < 2^31)
+template <typename A, typename F>
+__device__ A cov_pairwise(const F& term, int n) {
+  if (n <= 128) return cov_leaf<A>(term, 0, n);
   int off[32], len[32];
   unsigned char phase[32];
   A vals[32];
@@ -98,7 +122,7 @@ __device__ A cov_pairwise(const T* __restrict__ x, int n) {
     const int top = sp - 1;
     const int o = off[top], l = len[top];
     if (l <= 128) {
-      vals[vp++] = cov_leaf<A, T>(x + o, l);
+      vals[vp++] = cov_leaf<A>(term, o, l);
       sp--;
       continue;
     }
@@ -121,13 +145,48 @@ __device__ A cov_pairwise(const T* __restrict__ x, int n) {
 
 template <typename T>
 __global__ void cov_location_1d_kernel(const T* __restrict__ x, int64_t n, T* __restrict__ loc,
-                                       double* __restrict__ mean, int32_t* __restrict__ flags) {
+                                       double* __restrict__ mean, T* __restrict__ var, int32_t* __restrict__ flags) {
   int flag = 0;
   for (int64_t i = 0; i < n; i++) flag |= cov_flag((double)x[i]);
   // the reduce adds the pairwise sum to the identity 0 (this also turns a -0 sum into +0, as NumPy does)
-  loc[0] = cov_div<T>(Rn<T>::add((T)0, cov_pairwise<T, T>(x, (int)n)), n);
-  mean[0] = __ddiv_rn(__dadd_rn(0.0, cov_pairwise<double, T>(x, (int)n)), (double)n);
+  const T m = cov_div<T>(Rn<T>::add((T)0, cov_pairwise<T>([&](int i) { return x[i]; }, (int)n)), n);
+  if (loc) loc[0] = m;
+  mean[0] = __ddiv_rn(__dadd_rn(0.0, cov_pairwise<double>([&](int i) { return (double)x[i]; }, (int)n)), (double)n);
   *flags = flag;
+  if (var) {
+    const auto sq = [&](int i) {
+      const T e = Rn<T>::sub(x[i], m);
+      return Rn<T>::mul(e, e);
+    };
+    var[0] = cov_div<T>(Rn<T>::add((T)0, cov_pairwise<T>(sq, (int)n)), n);
+  }
+}
+
+static int cov_moments(const void* x, int dtype, int64_t n, int64_t d, void* location, double* mean, void* var,
+                       int32_t* flags, void* stream) {
+  TIP_REQUIRE(dtype == TIP_F32 || dtype == TIP_F64, "dtype must be TIP_F32 or TIP_F64");
+  TIP_REQUIRE(n >= 1 && n < (1LL << 31) && d >= 1 && d <= 65536, "shape");
+  TIP_REQUIRE(x && mean && flags, "null pointer");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (d == 1) {
+    if (dtype == TIP_F32)
+      cov_location_1d_kernel<float><<<1, 1, 0, st>>>((const float*)x, n, (float*)location, mean, (float*)var, flags);
+    else
+      cov_location_1d_kernel<double><<<1, 1, 0, st>>>((const double*)x, n, (double*)location, mean, (double*)var,
+                                                      flags);
+    TIP_LAUNCH_CHECK();
+    return TIP_OK;
+  }
+  TIP_CHECK_CUDA(cudaMemsetAsync(flags, 0, sizeof(int32_t), st));
+  const unsigned grid = (unsigned)((d + kCovThreads - 1) / kCovThreads);
+  if (dtype == TIP_F32)
+    cov_location_kernel<float><<<grid, kCovThreads, 0, st>>>((const float*)x, n, d, (float*)location, mean,
+                                                             (float*)var, flags);
+  else
+    cov_location_kernel<double><<<grid, kCovThreads, 0, st>>>((const double*)x, n, d, (double*)location, mean,
+                                                              (double*)var, flags);
+  TIP_LAUNCH_CHECK();
+  return TIP_OK;
 }
 
 }  // namespace tip
@@ -136,24 +195,12 @@ using namespace tip;
 
 extern "C" int tip_cov_location(const void* x, int dtype, int64_t n, int64_t d, void* location, double* mean,
                                 int32_t* flags, void* stream) {
-  TIP_REQUIRE(dtype == TIP_F32 || dtype == TIP_F64, "dtype must be TIP_F32 or TIP_F64");
-  TIP_REQUIRE(n >= 1 && n < (1LL << 31) && d >= 1 && d <= 65536, "shape");
-  TIP_REQUIRE(x && location && mean && flags, "null pointer");
-  cudaStream_t st = (cudaStream_t)stream;
-  if (d == 1) {
-    if (dtype == TIP_F32)
-      cov_location_1d_kernel<float><<<1, 1, 0, st>>>((const float*)x, n, (float*)location, mean, flags);
-    else
-      cov_location_1d_kernel<double><<<1, 1, 0, st>>>((const double*)x, n, (double*)location, mean, flags);
-    TIP_LAUNCH_CHECK();
-    return TIP_OK;
-  }
-  TIP_CHECK_CUDA(cudaMemsetAsync(flags, 0, sizeof(int32_t), st));
-  const unsigned grid = (unsigned)((d + kCovThreads - 1) / kCovThreads);
-  if (dtype == TIP_F32)
-    cov_location_kernel<float><<<grid, kCovThreads, 0, st>>>((const float*)x, n, d, (float*)location, mean, flags);
-  else
-    cov_location_kernel<double><<<grid, kCovThreads, 0, st>>>((const double*)x, n, d, (double*)location, mean, flags);
-  TIP_LAUNCH_CHECK();
-  return TIP_OK;
+  TIP_REQUIRE(location, "null pointer");
+  return cov_moments(x, dtype, n, d, location, mean, nullptr, flags, stream);
+}
+
+extern "C" int tip_col_var(const void* x, int dtype, int64_t n, int64_t d, void* var, double* mean, int32_t* flags,
+                           void* stream) {
+  TIP_REQUIRE(var, "null pointer");
+  return cov_moments(x, dtype, n, d, nullptr, mean, var, flags, stream);
 }

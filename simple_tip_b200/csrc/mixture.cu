@@ -9,7 +9,9 @@
 //
 //   gmm_quad_kernel     q[k, i] = |(x_i - mu_k) . L_k|^2 (L_k upper triangular): 64 x 64 output tiles of Y on DMMA,
 //                       the zero blocks of the triangle skipped, squared and row-summed in the epilogue (Y is never
-//                       stored); one CTA walks all column blocks of its 64 rows in ascending order
+//                       stored); one CTA walks all column blocks of its 64 rows in ascending order.  Its store
+//                       variant (kLower) is LSA's training-row whitening (x[:, cols] - mu) . W, W lower triangular,
+//                       written as fp32
 //   gmm_resp_kernel     log w_k - (D log 2pi + q) / 2 + log det L_k, log-sum-exp over k, resp = exp(. - lse), block
 //                       partials of sum(lse) (merged by gmm_mean_kernel in ascending block order)
 //   gmm_moments_kernel  per row chunk: sum_i r_ik and sum_i r_ik x_i (merged by gmm_moments_finish_kernel, which
@@ -75,16 +77,23 @@ __device__ __forceinline__ void gm_zero(double acc[2][4][4]) {
       for (int i = 0; i < 4; i++) acc[mt][nt][i] = 0.0;
 }
 
-// ---- E-step quadratic forms -----------------------------------------------------------------------------------
-// grid (row tiles, K).  Y = (X - mu_k) . L_k tile by tile: column block j0 needs the rows l < j0 + 64 of L only,
-// and inside the diagonal block the entries below the diagonal are read as 0.  Epilogue: per (row, column block)
-// the 64 squares summed in double (thread: its 8 columns in order; quad: xor butterfly; the two column halves:
-// left + right), accumulated over the column blocks in ascending order.
-template <typename T>
+// ---- E-step quadratic forms / LSA's training-row whitening -----------------------------------------------------
+// grid (row tiles, K).  Y = (X - mu_k) . L_k tile by tile.
+// kLower == false (E-step): L_k is upper triangular, so column block j0 needs the rows l < j0 + 64 of L only, and
+//   inside the diagonal block the entries below the diagonal are read as 0.  Epilogue: per (row, column block) the
+//   64 squares summed in double (thread: its 8 columns in order; quad: xor butterfly; the two column halves: left +
+//   right), accumulated over the column blocks in ascending order.
+// kLower == true (LSA whitening, scipy 1.4.1's points . cholesky(inv_cov)): L is lower triangular, so column block
+//   j0 needs the rows l >= j0 only (the mirror skip), and inside the diagonal block the entries above the diagonal are
+//   read as 0.  X's columns are read through the column list cols (NULL: 0..d-1) of rows of ld entries, and Y is
+//   stored as fp32, rounded once from the float64 accumulator.
+template <typename T, bool kLower>
 __global__ void __launch_bounds__(kGmThreads) gmm_quad_kernel(const T* __restrict__ x, int64_t n, int d,
                                                               const double* __restrict__ mu,
                                                               const double* __restrict__ chol,
-                                                              double* __restrict__ q) {
+                                                              double* __restrict__ q, int64_t ld,
+                                                              const int32_t* __restrict__ cols,
+                                                              float* __restrict__ y) {
   __shared__ GmTile s;
   __shared__ double s_half[2][kGmBM];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
@@ -93,51 +102,75 @@ __global__ void __launch_bounds__(kGmThreads) gmm_quad_kernel(const T* __restric
   const int k = blockIdx.y;
   const double* muk = mu + (int64_t)k * d;
   const double* L = chol + (int64_t)k * d * d;
+  if (!kLower) ld = d;
   double total = 0.0;   // thread tid < 64: row i0 + tid
   double acc[2][4][4];
   for (int j0 = 0; j0 < d; j0 += kGmBN) {
     gm_zero(acc);
-    const int lend = min(d, j0 + kGmBN);
-    for (int l0 = 0; l0 < lend; l0 += kGmBK) {
+    const int lbeg = kLower ? j0 : 0, lend = kLower ? d : min(d, j0 + kGmBN);
+    for (int l0 = lbeg; l0 < lend; l0 += kGmBK) {
       __syncthreads();
       for (int e = tid; e < kGmBM * kGmBK; e += kGmThreads) {   // centred rows, widened to double
         const int r = e / kGmBK, l = e % kGmBK;
         const int64_t i = i0 + r;
         double v = 0.0;
-        if (i < n && l0 + l < d) v = (double)x[i * d + l0 + l] - muk[l0 + l];
+        if (i < n && l0 + l < d) {
+          const int64_t src = (kLower && cols) ? (int64_t)cols[l0 + l] : (int64_t)(l0 + l);
+          v = (double)x[i * ld + src] - muk[l0 + l];
+        }
         s.a[l][r] = v;
       }
       for (int e = tid; e < kGmBK * kGmBN; e += kGmThreads) {
         const int l = e / kGmBN, j = e % kGmBN;
         const int gl = l0 + l, gj = j0 + j;
-        s.b[l][j] = (gj < d && gl <= gj) ? L[(int64_t)gl * d + gj] : 0.0;
+        const bool inside = kLower ? (gl < d && gj < d && gl >= gj) : (gj < d && gl <= gj);
+        s.b[l][j] = inside ? L[(int64_t)gl * d + gj] : 0.0;
       }
       __syncthreads();
       gm_tile_step(s, acc, wm, wn, g, t);
     }
+    if constexpr (kLower) {
+      // staged through the operand tiles (64 x 64 floats fit in one of them), then stored row by row
+      float* stage = reinterpret_cast<float*>(&s.a[0][0]);
+      __syncthreads();
 #pragma unroll
-    for (int mt = 0; mt < 2; mt++) {
-      double r0 = 0.0, r1 = 0.0;
+      for (int mt = 0; mt < 2; mt++)
 #pragma unroll
-      for (int nt = 0; nt < 4; nt++) {
-        r0 = fma(acc[mt][nt][0], acc[mt][nt][0], r0);
-        r0 = fma(acc[mt][nt][1], acc[mt][nt][1], r0);
-        r1 = fma(acc[mt][nt][2], acc[mt][nt][2], r1);
-        r1 = fma(acc[mt][nt][3], acc[mt][nt][3], r1);
+        for (int nt = 0; nt < 4; nt++)
+#pragma unroll
+          for (int h = 0; h < 4; h++)
+            stage[(wm * 32 + mt * 16 + g + 8 * (h >> 1)) * kGmBN + wn * 32 + nt * 8 + 2 * t + (h & 1)] =
+                __double2float_rn(acc[mt][nt][h]);
+      __syncthreads();
+      for (int e = tid; e < kGmBM * kGmBN; e += kGmThreads) {
+        const int r = e / kGmBN, j = e % kGmBN;
+        if (i0 + r < n && j0 + j < d) y[(i0 + r) * d + j0 + j] = stage[e];
       }
-      r0 += __shfl_xor_sync(0xffffffffu, r0, 1);
-      r0 += __shfl_xor_sync(0xffffffffu, r0, 2);
-      r1 += __shfl_xor_sync(0xffffffffu, r1, 1);
-      r1 += __shfl_xor_sync(0xffffffffu, r1, 2);
-      if (t == 0) {
-        s_half[wn][wm * 32 + mt * 16 + g] = r0;
-        s_half[wn][wm * 32 + mt * 16 + g + 8] = r1;
+    } else {
+#pragma unroll
+      for (int mt = 0; mt < 2; mt++) {
+        double r0 = 0.0, r1 = 0.0;
+#pragma unroll
+        for (int nt = 0; nt < 4; nt++) {
+          r0 = fma(acc[mt][nt][0], acc[mt][nt][0], r0);
+          r0 = fma(acc[mt][nt][1], acc[mt][nt][1], r0);
+          r1 = fma(acc[mt][nt][2], acc[mt][nt][2], r1);
+          r1 = fma(acc[mt][nt][3], acc[mt][nt][3], r1);
+        }
+        r0 += __shfl_xor_sync(0xffffffffu, r0, 1);
+        r0 += __shfl_xor_sync(0xffffffffu, r0, 2);
+        r1 += __shfl_xor_sync(0xffffffffu, r1, 1);
+        r1 += __shfl_xor_sync(0xffffffffu, r1, 2);
+        if (t == 0) {
+          s_half[wn][wm * 32 + mt * 16 + g] = r0;
+          s_half[wn][wm * 32 + mt * 16 + g + 8] = r1;
+        }
       }
+      __syncthreads();
+      if (tid < kGmBM) total += s_half[0][tid] + s_half[1][tid];
     }
-    __syncthreads();
-    if (tid < kGmBM) total += s_half[0][tid] + s_half[1][tid];
   }
-  if (tid < kGmBM && i0 + tid < n) q[(int64_t)k * n + i0 + tid] = total;
+  if (!kLower && tid < kGmBM && i0 + tid < n) q[(int64_t)k * n + i0 + tid] = total;
 }
 
 // ---- responsibilities, log-sum-exp, lower bound ---------------------------------------------------------------
@@ -389,9 +422,30 @@ extern "C" int tip_gmm_quad(const void* x, int dtype, int64_t n, int64_t d, cons
   const dim3 grid((unsigned)((n + kGmBM - 1) / kGmBM), (unsigned)k);
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype == TIP_F32)
-    gmm_quad_kernel<float><<<grid, kGmThreads, 0, st>>>((const float*)x, n, (int)d, means, prec_chol, q);
+    gmm_quad_kernel<float, false><<<grid, kGmThreads, 0, st>>>((const float*)x, n, (int)d, means, prec_chol, q, d,
+                                                               nullptr, nullptr);
   else
-    gmm_quad_kernel<double><<<grid, kGmThreads, 0, st>>>((const double*)x, n, (int)d, means, prec_chol, q);
+    gmm_quad_kernel<double, false><<<grid, kGmThreads, 0, st>>>((const double*)x, n, (int)d, means, prec_chol, q, d,
+                                                                nullptr, nullptr);
+  TIP_LAUNCH_CHECK();
+  return TIP_OK;
+}
+
+extern "C" int tip_whiten_dmma(const void* x, int dtype, int64_t m, int64_t d_in, const int32_t* cols, int64_t d_out,
+                               const double* mu, const double* w_lower, float* out, void* stream) {
+  TIP_REQUIRE(dtype == TIP_F32 || dtype == TIP_F64, "dtype must be TIP_F32 or TIP_F64");
+  int rc = gm_check(m, d_out, 1);
+  if (rc != TIP_OK) return rc;
+  TIP_REQUIRE(d_in >= d_out && (cols || d_in == d_out), "shape");
+  TIP_REQUIRE(x && mu && w_lower && out, "null pointer");
+  const dim3 grid((unsigned)((m + kGmBM - 1) / kGmBM), 1u);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (dtype == TIP_F32)
+    gmm_quad_kernel<float, true><<<grid, kGmThreads, 0, st>>>((const float*)x, m, (int)d_out, mu, w_lower, nullptr,
+                                                              d_in, cols, out);
+  else
+    gmm_quad_kernel<double, true><<<grid, kGmThreads, 0, st>>>((const double*)x, m, (int)d_out, mu, w_lower, nullptr,
+                                                               d_in, cols, out);
   TIP_LAUNCH_CHECK();
   return TIP_OK;
 }

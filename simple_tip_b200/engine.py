@@ -1135,8 +1135,9 @@ F16_NORM_SCALE = 64.0       # tail scale of the fp16 operand: |p|^2 / 2 / 64 mus
 
 
 class KdeEngine:
-    def __init__(self, p_whitened: np.ndarray, comm: Optional[TrainShardComm] = None):
-        """p_whitened: [n, d] float64 whitened, centred training traces (host).  With a communicator
+    def __init__(self, p_whitened, comm: Optional[TrainShardComm] = None):
+        """p_whitened: [n, d] whitened, centred training traces: float64 on the host, or fp32 on the device (the
+        device KDE fit's tip_whiten_dmma output; used in place).  With a communicator
         of more than one rank the engine keeps rows rank::world (N_train sharded) and merges the
         per-shard partial sums in log_kernel_sum (north_star: one exchange of partial KDE sums).
 
@@ -1148,7 +1149,9 @@ class KdeEngine:
         self.lib = _lib.load()
         self.comm = comm if (comm is not None and comm.world > 1) else None
         if self.comm is not None:
-            p_whitened = np.ascontiguousarray(p_whitened[self.comm.rank::self.comm.world])
+            p_whitened = p_whitened[self.comm.rank::self.comm.world]
+            if isinstance(p_whitened, np.ndarray):
+                p_whitened = np.ascontiguousarray(p_whitened)
         self.n, self.d = p_whitened.shape
         self.precision = "split-bf16 x3 (h.h + h.l + l.h, ~2^-17 relative)"
         self.pitch = int(self.lib.tip_pair_pitch(self.d, 3))
@@ -1156,7 +1159,10 @@ class KdeEngine:
         sms = C.c_int(0)
         _lib.check(self.lib.tip_device_info(C.byref(sms), None, None), "tip_device_info")
         self.sms = sms.value
-        p32 = to_device(p_whitened.astype(np.float32), self.dev)
+        if isinstance(p_whitened, torch.Tensor):
+            p32 = p_whitened.to(self.dev, torch.float32).contiguous()
+        else:
+            p32 = to_device(p_whitened.astype(np.float32), self.dev)
         self.t_pack = torch.empty((self.n, self.pitch), dtype=torch.bfloat16, device=self.dev)
         _lib.check(self.lib.tip_pair_prep(_p(p32), _lib.TIP_F32, self.n, self.d, None, _lib.ROLE_TRAIN, 3, 1.0, -0.5,
                                           _p(self.t_pack), None, None, _stream()), "tip_pair_prep")
@@ -1594,6 +1600,164 @@ def cov_scores(x: torch.Tensor, fit: dict) -> torch.Tensor:
         return torch.zeros(x.shape[0], dtype=torch.float64, device=x.device)
     cols = fit["live"].to(torch.int32)
     return quadratic_forms(x, [(fit["score_mu"], fit["score_w"])], cols)[0]
+
+
+# ------------------------------------------------------------------------------------------
+# LSA's fit (surprise.py:417-437 + StableGaussianKDE, stable_kde.py:20-77): column variances, KDE fit
+# ------------------------------------------------------------------------------------------
+def col_var(x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """(var [d] x.dtype = np.var(x, axis=0) bit for bit, float64 column mean [d], non-finite flags [1] int32: bit 0
+    NaN, bit 1 inf) of the [n, d] device matrix x, all on the device."""
+    lib = _lib.load()
+    n, d = x.shape
+    var = torch.empty(d, dtype=x.dtype, device=x.device)
+    mean = torch.empty(d, dtype=torch.float64, device=x.device)
+    flags = torch.empty(1, dtype=torch.int32, device=x.device)
+    _lib.check(lib.tip_col_var(_p(x), tip_dtype(x.dtype), n, d, _p(var), _p(mean), _p(flags), _stream()),
+               "tip_col_var")
+    return var, mean, flags
+
+
+def whiten_f64(x: torch.Tensor, cols: Optional[torch.Tensor], mu: torch.Tensor, w_lower: torch.Tensor) -> torch.Tensor:
+    """(x[:, cols] - mu) @ w_lower as fp32 [m, d'], accumulated in float64 on the fp64 tensor cores (tip_whiten_dmma);
+    cols int32 [d'] or None, mu float64 [d'], w_lower float64 [d', d'] lower triangular."""
+    lib = _lib.load()
+    m, d_in = x.shape
+    d = w_lower.shape[0]
+    out = torch.empty((m, d), dtype=torch.float32, device=x.device)
+    _lib.check(lib.tip_whiten_dmma(_p(x), tip_dtype(x.dtype), m, d_in, _p(cols), d, _p(mu), _p(w_lower), _p(out),
+                                   _stream()), "tip_whiten_dmma")
+    return out
+
+
+KDE_MAX_INCREMENT = 1e-5
+KDE_NOT_FIXED = ("Was not able to fix numerical imprecision in covariance matrix."
+                 "Failing silently. All likelihoods will be reported as 0.")
+
+
+def kde_cov_fact(n: int) -> float:
+    """np.cov(X, bias=False, aweights=ones(n)/n)'s normalisation, with np.cov's own expressions (warning as np.cov
+    does when it is not positive): fact = w_sum - ddof * sum(w * aweights) / w_sum, ddof = 1."""
+    import warnings
+
+    w = np.ones(n) / n
+    w_sum = np.broadcast_to(w, (1, n)).sum(axis=1, dtype=np.float64)[0]      # np.average's scl
+    fact = w_sum - 1 * np.sum(w * w) / w_sum
+    if fact <= 0:
+        warnings.warn("Degrees of freedom <= 0 for slice", RuntimeWarning, stacklevel=3)
+        fact = 0.0
+    return fact
+
+
+def kde_fit(x: torch.Tensor, cols: Optional[np.ndarray] = None, mean: Optional[torch.Tensor] = None,
+            timing: Optional[dict] = None) -> dict:
+    """StableGaussianKDE(x[:, cols].T)'s fit (scott bandwidth, uniform weights) on the [n, D] device matrix x
+    (float32 / float64), in float64 on the device:
+    - covariance: np.cov(bias=False, aweights=1/n) = the DMMA scatter of tip_gmm_scatter (k = 1, resp = 1/n) of the
+      kept columns (one index_select), centred on their float64 column mean (`mean` [D], from col_var, or computed
+      here), times np.true_divide(1, fact) with np.cov's fact;
+    - the stabilisation loop: while some eigenvalue (eigvalsh) of cov * factor^2 is <= d' eps max|lambda|, the
+      diagonal is REPLACED by 1e-10 * 2^k; past 1e-5 the fit fails silently (prepare_failed, warning);
+    - inv (inv_ex: a singular matrix sets prepare_failed), cholesky(2 pi covariance) for log_det, det for
+      _norm_factor, W = cholesky(inv_cov) (cholesky_ex: failure raises NumPy's LinAlgError);
+    - p = (x[:, cols] - mu) @ W as fp32 (tip_whiten_dmma), the operand of KdeEngine.
+    A non-finite covariance raises LinAlgError("Eigenvalues did not converge"), as the host's eigh does.  Returns a
+    dict of device tensors (rows = x[:, cols], covariance (unscaled, stabilised), inv (of it), whitening, mean [d'],
+    p) and host values (diag_w, the whitening's diagonal, n, d, factor, rounds, prepare_failed, log_det,
+    norm_factor); a failed fit has none of the entries from covariance on.  timing: receives CUDA-event milliseconds
+    (col_var (when mean is None), scatter, factor, whiten, total) and the read-back count."""
+    import warnings
+
+    n, width = x.shape
+    dev = x.device
+    cols_t = None if cols is None else torch.from_numpy(np.ascontiguousarray(cols, dtype=np.int64)).to(dev)
+    d = width if cols is None else int(cols_t.shape[0])
+    marks = {}
+
+    def mark(key):
+        if timing is not None:
+            marks[key] = torch.cuda.Event(enable_timing=True)
+            marks[key].record()
+
+    mark("start")
+    if mean is None:
+        _, mean, _ = col_var(x)
+        mark("col_var")
+    xs = x if cols_t is None else x.index_select(1, cols_t)
+    mu = mean if cols_t is None else mean.index_select(0, cols_t)
+    mu = mu.contiguous()
+    resp = torch.full((1, n), 1.0 / n, dtype=torch.float64, device=dev)        # np.ones(n) / n
+    inv_fact = float(np.true_divide(1, kde_cov_fact(n)))
+    cov = gmm_scatter(xs.contiguous(), resp, mu.reshape(1, d))[0] * inv_fact
+    mark("scatter")
+    w = np.ones(n) / n
+    neff = 1.0 / np.sum(w ** 2)
+    factor = float(np.power(neff, -1.0 / (d + 4)))
+    f2 = factor ** 2
+    eps = np.finfo(np.float64).eps
+    increment, rounds, failed, reads = 1e-10, 0, False, 0
+    while True:
+        try:
+            lam = torch.linalg.eigvalsh(cov * f2)
+        except torch.linalg.LinAlgError:             # e.g. NaN / inf entries: NumPy's eigh raises this
+            raise np.linalg.LinAlgError("Eigenvalues did not converge") from None
+        thr = d * eps * lam.abs().max()
+        state = torch.stack([(lam <= thr).any().to(torch.float64), torch.isfinite(cov).all().to(torch.float64)]).cpu()
+        rounds, reads = rounds + 1, reads + 1
+        if state[1] == 0:
+            raise np.linalg.LinAlgError("Eigenvalues did not converge")
+        if state[0] == 0:
+            break
+        cov.fill_diagonal_(increment)
+        if increment > KDE_MAX_INCREMENT:
+            warnings.warn(KDE_NOT_FIXED)
+            failed = True
+            break
+        increment += increment
+    out = {"n": n, "d": d, "factor": factor, "rounds": rounds, "prepare_failed": failed, "mean": mu, "rows": xs}
+    if failed:
+        mark("factor")
+        _finish_timing(timing, marks, reads)
+        return out
+    inv, info_inv = torch.linalg.inv_ex(cov)
+    covariance = cov * f2
+    inv_cov = inv / f2
+    chol, info_c = torch.linalg.cholesky_ex(covariance * 2 * np.pi)
+    log_det = 2 * torch.log(torch.diagonal(chol)).sum()
+    norm_factor = torch.sqrt(torch.linalg.det(2 * np.pi * covariance))
+    wl, info_w = torch.linalg.cholesky_ex(inv_cov)
+    wl = wl.contiguous()                           # row-major, as the kernels and the query whitening read it
+    diag_w = torch.diagonal(wl)
+    host = torch.cat([torch.stack([info_inv.to(torch.float64), info_c.to(torch.float64), info_w.to(torch.float64),
+                                   log_det, norm_factor]), diag_w]).cpu().numpy()
+    reads += 1
+    mark("factor")
+    if host[0] != 0:                               # np.linalg.inv raised LinAlgError: the host sets prepare_failed
+        out["prepare_failed"] = True
+        _finish_timing(timing, marks, reads)
+        return out
+    if host[1] != 0 or host[2] != 0:
+        raise np.linalg.LinAlgError("Matrix is not positive definite")
+    cols32 = None if cols_t is None else cols_t.to(torch.int32)
+    p = whiten_f64(x, cols32, mu, wl)
+    mark("whiten")
+    _finish_timing(timing, marks, reads)
+    out.update({"covariance": cov, "inv": inv, "whitening": wl, "p": p, "diag_w": host[5:],
+                "log_det": float(host[3]), "norm_factor": float(host[4])})
+    return out
+
+
+def _finish_timing(timing: Optional[dict], marks: dict, reads: int):
+    if timing is None:
+        return
+    marks["end"] = torch.cuda.Event(enable_timing=True)
+    marks["end"].record()
+    torch.cuda.synchronize()
+    keys = list(marks)
+    for a, b in zip(keys[:-2], keys[1:-1]):
+        timing[b] = timing.get(b, 0.0) + marks[a].elapsed_time(marks[b])
+    timing["total"] = timing.get("total", 0.0) + marks["start"].elapsed_time(marks["end"])
+    timing["reads"] = timing.get("reads", 0) + reads
 
 
 def silhouette_samples(x: torch.Tensor, labels: torch.Tensor, n_clusters: int,
