@@ -12,6 +12,10 @@
  *
  * Which reference arithmetic each entry point replaces (paths relative to the reference):
  *   tip_deepgini        src/core/deepgini.py:31-35     argmax + 1 - sum(p*p)
+ *   tip_softmax_stat    handler_model.py:23-85 uwiz MaxSoftmax / PredictionConfidenceScore / SoftmaxEntropy
+ *                       (and DeepGini) on softmax outputs
+ *   tip_vote_add        handler_model.py:148-166 uwiz VariationRatio: argmax votes of MC-dropout samples,
+ *   tip_vote_finish     streamed pass by pass; mode and 1 - votes / samples
  *   tip_kmnc            src/core/neuron_coverage.py:82-94 (+ sum_score :8-22)
  *   tip_cam_buckets     src/core/prioritizers.py:16-45 (greedy loop of cam) on compact KMNC profiles
  *   tip_pair_prep       (new) operand packing for the tensor-core pass
@@ -102,6 +106,32 @@ uint64_t tip_launch_count(void);
  * input dtype, summed in NumPy's pairwise order (bit-identical to np.sum(p*p, axis=1)). */
 int tip_deepgini(const void* probs, int dtype, int64_t n, int64_t c, int32_t* pred, void* gini,
                  void* stream);
+
+/* ---- uncertainty quantifiers of uncertainty-wizard 0.2.0 (handler_model.py:23-85,102-173) -----
+ * tip_softmax_stat: probs n x c (TIP_F32 or TIP_F64); pred[n] = first argmax, out[n] in the input dtype:
+ *   TIP_STAT_GINI     1 - sum(p*p), the same as tip_deepgini
+ *   TIP_STAT_MAX      max(p)                                        MaxSoftmax
+ *   TIP_STAT_PCS      top-1 minus top-2 of p (0 for a repeated max) PredictionConfidenceScore; needs c >= 2
+ *   TIP_STAT_ENTROPY  -sum(q*log2(q)), q = p with exact zeros replaced by 1e-20   SoftmaxEntropy
+ * GINI, MAX and PCS are bit-identical to NumPy; ENTROPY sums in NumPy's pairwise order, its log2 is within an
+ * ulp of libm's.  The values are uncertainties or confidences as the quantifier defines them, unsigned.
+ *
+ * tip_vote_add: the argmax (first index) of every sampled row, added to counts[n x c] (int32, zeroed by the
+ * caller before the first call).  Sample s of row i is the c-vector at probs + i*row_stride + s*sample_stride
+ * (elements); dense [n, samples, c] input is sample_stride = c, row_stride = samples*c.  Calls accumulate, so
+ * samples may arrive in chunks (MC-dropout passes).
+ * tip_vote_finish: pred[n] = the lowest class with the most votes (scipy.stats.mode), vr[n] = 1 - votes/samples
+ * (float64)                                                        VariationRatio */
+#define TIP_STAT_GINI 0
+#define TIP_STAT_MAX 1
+#define TIP_STAT_PCS 2
+#define TIP_STAT_ENTROPY 3
+int tip_softmax_stat(const void* probs, int dtype, int64_t n, int64_t c, int kind, int32_t* pred, void* out,
+                     void* stream);
+int tip_vote_add(const void* probs, int dtype, int64_t n, int64_t c, int64_t samples, int64_t sample_stride,
+                 int64_t row_stride, int32_t* counts, void* stream);
+int tip_vote_finish(const int32_t* counts, int64_t n, int64_t c, int64_t samples, int32_t* pred, double* vr,
+                    void* stream);
 
 /* ---- KMNC (neuron_coverage.py:65-94) -------------------------------------------------
  * act: n x d (TIP_F32/TIP_F64); mins, jumps: d values of stat_dtype, jumps = (max-min)/k

@@ -19,6 +19,7 @@ CAM_MAX_BLOCKS = 1024
 ROLE_QUERY, ROLE_TRAIN = 0, 1
 RANGE_SAME_CLASS, RANGE_OTHER_CLASSES = 0, 1
 ROW_TILE, COL_TILE = 128, 256
+STAT_GINI, STAT_MAX, STAT_PCS, STAT_ENTROPY = 0, 1, 2, 3
 
 
 class RerankExtras(C.Structure):
@@ -43,6 +44,9 @@ _SIGNATURES = {
     "tip_device_info": (C.c_int, [C.POINTER(C.c_int)] * 3),
     "tip_launch_count": (C.c_uint64, []),
     "tip_deepgini": (C.c_int, [_vp, C.c_int, _i64, _i64, _vp, _vp, _vp]),
+    "tip_softmax_stat": (C.c_int, [_vp, C.c_int, _i64, _i64, C.c_int, _vp, _vp, _vp]),
+    "tip_vote_add": (C.c_int, [_vp, C.c_int, _i64, _i64, _i64, _i64, _i64, _vp, _vp]),
+    "tip_vote_finish": (C.c_int, [_vp, _i64, _i64, _i64, _vp, _vp, _vp]),
     "tip_kmnc": (C.c_int, [_vp, C.c_int, _i64, _i64, _vp, _vp, C.c_int, _i32, _vp, C.c_int, _vp, _vp]),
     "tip_cam_buckets": (C.c_int, [_vp, C.c_int, _i64, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _vp]),
     "tip_cover_packed_words": (_i64, [_i64]),

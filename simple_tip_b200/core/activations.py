@@ -97,6 +97,117 @@ class TransparentModel:
         return [torch.cat(lst, dim=0) for lst in per_layer]
 
 
+DROPOUT_SAMPLE_SIZE = 200      # handler_model.py:7
+MC_ROWS_PER_PASS = 8192        # rows of one MC-dropout forward pass: a batch is replicated up to this many
+
+
+def get_pred_and_uncertainty(model, x, batch_size: int = 32, sample_size: int = DROPOUT_SAMPLE_SIZE, seed: int = 0
+                             ) -> Tuple[np.ndarray, Dict[str, np.ndarray], Dict[str, List[float]]]:
+    """Point predictions and uncertainties of a torch model (handler_model.py:102-173, `BaseModel.get_pred_and_uncertainty`).
+
+    The model's output is taken to be its softmax output, as in the study, whose models end in a softmax layer; wrap
+    a model that returns logits (e.g. `torch.nn.Sequential(model, torch.nn.Softmax(dim=1))`) before calling this.
+
+    Returns (pred, uncertainties, times) like the reference: pred is the argmax of the point pass (int64);
+    uncertainties holds "softmax", "pcs", "softmax_entropy" and "deep_gini" as stored by the study
+    (`as_confidence=False`: the max softmax and PCS are negated) and, when the model has dropout modules, "VR", the
+    variation ratio over `sample_size` MC-dropout samples; times[name] = [0, prediction time, quantifier time, 0]
+    in seconds.  `x` must hold at least one input (ValueError otherwise).
+
+    The model runs wherever its parameters live (the host, or any CUDA device); `x` is moved there.  Its outputs
+    are scored on the current CUDA device: they are copied there when the model lives elsewhere.
+
+    The point pass runs in eval mode without gradients.  The MC-dropout passes switch only the dropout modules
+    (`torch.nn.modules.dropout._DropoutNd`) to training mode — batch norm and everything else stays in eval mode —
+    and restore every module's mode afterwards.  Each batch of `batch_size` inputs is replicated along the batch
+    dimension up to MC_ROWS_PER_PASS rows per forward pass; every pass's votes go straight to `tip_vote_add`, so
+    the [N, sample_size, C] samples are never held at once.  Memory: one pass holds MC_ROWS_PER_PASS replicated
+    inputs plus the model's activations for them — 8192 rows of 28 x 28 float32 are 26 MB, but of 3 x 224 x 224
+    3.9 GB before any activation; for large inputs pass a smaller `batch_size`, or a `sample_size` that keeps
+    batch_size x sample_size small (a batch is never split, so batch_size rows is the floor).  The passes draw
+    from torch's RNG seeded with `seed` inside `torch.random.fork_rng` (forking only the host's and the model
+    device's state), so results repeat and the caller's RNG state is untouched."""
+    import torch
+    from torch.nn.modules.dropout import _DropoutNd
+
+    from . import quantifiers as Q
+    from .deepgini import DeepGini
+    from .timer import Timer
+    from .. import engine as E
+
+    score_dev = E.require_cuda()
+    dev = next(iter(model.parameters()), torch.empty(0)).device
+    if not isinstance(x, torch.Tensor):
+        x = torch.from_numpy(np.ascontiguousarray(x))
+    if x.shape[0] == 0:
+        raise ValueError("x holds no inputs")
+    x = x.to(dev)
+
+    def synced(fn, timer):
+        with timer:
+            res = fn()
+            torch.cuda.synchronize(score_dev)
+            if dev.type == "cuda" and dev != score_dev:
+                torch.cuda.synchronize(dev)
+        return res
+
+    modes = [(m, m.training) for m in model.modules()]
+    uncertainties: Dict[str, np.ndarray] = {}
+    times: Dict[str, List[float]] = {}
+    try:
+        pred_timer = Timer()
+        probs = synced(lambda: TransparentModel(model, [], include_last_layer=True).collect(x, batch_size)[0],
+                       pred_timer)
+        pred = None
+        for q in (Q.MaxSoftmax, Q.PredictionConfidenceScore, Q.SoftmaxEntropy, DeepGini):
+            timer = Timer()
+            q_pred, values = synced(lambda: q.calculate(probs), timer)
+            if pred is None:
+                pred = q_pred
+            name = q.aliases()[0].replace("custom::", "")
+            uncertainties[name] = q.cast_conf_or_unc(False, values)
+            times[name] = [0, pred_timer.get(), timer.get(), 0]
+
+        dropouts = [m for m in model.modules() if isinstance(m, _DropoutNd)]
+        if dropouts:
+            n, c = probs.shape
+            votes = Q.Votes(n, c, score_dev)
+            sampling_timer, vote_timer = Timer(), Timer()
+            model.eval()
+            for m in dropouts:
+                m.train()
+            with torch.random.fork_rng(devices=[dev] if dev.type == "cuda" else []), torch.no_grad():
+                torch.default_generator.manual_seed(seed)
+                if dev.type == "cuda":
+                    with torch.cuda.device(dev):
+                        torch.cuda.manual_seed(seed)
+                for start in range(0, n, batch_size):
+                    xb = x[start:start + batch_size]
+                    b = xb.shape[0]
+                    done = 0
+                    while done < sample_size:
+                        r = min(sample_size - done, max(1, MC_ROWS_PER_PASS // b))
+                        # row i * r + j of the pass is replica j of input i: [b, r, C] once viewed
+                        xr = xb.unsqueeze(1).expand(b, r, *xb.shape[1:]).reshape(b * r, *xb.shape[1:])
+                        out = synced(lambda: model(xr).detach(), sampling_timer)
+                        if tuple(out.shape) != (b * r, c):
+                            raise ValueError(f"an MC-dropout pass returned {tuple(out.shape)}, expected {(b * r, c)}")
+
+                        def vote():
+                            o = out if out.dtype in (torch.float32, torch.float64) else out.to(torch.float32)
+                            votes.add(E.to_device(o, score_dev), r, sample_stride=c, row_stride=r * c, row0=start,
+                                      rows=b)
+                        synced(vote, vote_timer)
+                        done += r
+            _, vr = synced(lambda: votes.finish(sample_size), vote_timer)
+            uncertainties["VR"] = vr
+            times["VR"] = [0, sampling_timer.get(), vote_timer.get(), 0]
+    finally:
+        for m, training in modes:
+            m.training = training
+    return pred, uncertainties, times
+
+
 def _badge_dir(root: str, case_study: str, model_id: int, dataset: str) -> str:
     return os.path.join(root, "activations", case_study, f"model_{model_id}", dataset)
 

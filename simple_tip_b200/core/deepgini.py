@@ -56,21 +56,32 @@ class DeepGini(_Base):
         from .. import _lib
         from .. import engine as E
 
-        if isinstance(nn_outputs, torch.Tensor) and nn_outputs.is_cuda:     # softmax outputs already in HBM
-            p = nn_outputs if nn_outputs.dtype in (torch.float32, torch.float64) else nn_outputs.to(torch.float32)
-            p_np_dtype = E.NP_DTYPE[p.dtype]
-        else:
-            p = np.asarray(nn_outputs)
-            if p.dtype not in (np.float32, np.float64):
-                p = p.astype(np.float64)
-            p_np_dtype = p.dtype
-        assert p.ndim == 2, "nn_outputs must be (samples, classes)"
-        dev = E.require_cuda()
+        p_dev, p_np_dtype = device_probs(nn_outputs, 2)
         lib = _lib.load()
-        n, c = p.shape
-        p_dev = E.to_device(p, dev)
-        pred = torch.empty(n, dtype=torch.int32, device=dev)
-        gini = torch.empty(n, dtype=p_dev.dtype, device=dev)
+        n, c = p_dev.shape
+        pred = torch.empty(n, dtype=torch.int32, device=p_dev.device)
+        gini = torch.empty(n, dtype=p_dev.dtype, device=p_dev.device)
         _lib.check(lib.tip_deepgini(E._p(p_dev), E.tip_dtype(p_np_dtype), n, c, E._p(pred), E._p(gini), E._stream()),
                    "tip_deepgini")
         return pred.cpu().numpy().astype(np.int64), gini.cpu().numpy()
+
+
+def device_probs(nn_outputs, ndim: int):
+    """Softmax outputs as a contiguous float32 / float64 CUDA tensor, and their NumPy dtype.  CUDA tensors stay in
+    HBM (float16 / bfloat16 ones are widened to float32); host arrays keep float32 / float64 and are otherwise
+    widened to float64, then uploaded."""
+    import torch
+
+    from .. import engine as E
+
+    if isinstance(nn_outputs, torch.Tensor) and nn_outputs.is_cuda:     # softmax outputs already in HBM
+        p = nn_outputs if nn_outputs.dtype in (torch.float32, torch.float64) else nn_outputs.to(torch.float32)
+        p_np_dtype = E.NP_DTYPE[p.dtype]
+    else:
+        p = np.asarray(nn_outputs)
+        if p.dtype not in (np.float32, np.float64):
+            p = p.astype(np.float64)
+        p_np_dtype = p.dtype
+    assert p.ndim == ndim, "nn_outputs must be (samples, classes)" if ndim == 2 else \
+        "nn_outputs must be (samples, sample_size, classes)"
+    return E.to_device(p, E.require_cuda()), p_np_dtype

@@ -208,6 +208,89 @@ __device__ T np_sumsq_g8(const T* __restrict__ x, const T* __restrict__ y, int n
   return vals[0];
 }
 
+// ---- NumPy's pairwise order over an arbitrary per-element term -------------------------------
+// The leaf / split rules of np_leaf_sumsq / np_sumsq / np_leaf_sumsq_g8 above, with element i's term given by
+// term(i) (the softmax entropy sums q*log2(q)).  Kept apart from the (x-y)^2 routines, whose code the DSA re-rank
+// and DeepGini pin bit for bit, so that those compile exactly as before.
+template <typename T, typename F>
+__device__ __forceinline__ T np_leaf_sum_of(const F& term, int off, int n) {
+  using R = Rn<T>;
+  if (n < 8) {
+    T res = (T)0;
+    for (int i = 0; i < n; i++) res = R::add(res, term(off + i));
+    return res;
+  }
+  T r[8];
+#pragma unroll
+  for (int j = 0; j < 8; j++) r[j] = term(off + j);
+  int i = 8;
+  const int lim = n - (n % 8);
+  for (; i < lim; i += 8) {
+#pragma unroll
+    for (int j = 0; j < 8; j++) r[j] = R::add(r[j], term(off + i + j));
+  }
+  T res = R::add(R::add(R::add(r[0], r[1]), R::add(r[2], r[3])), R::add(R::add(r[4], r[5]), R::add(r[6], r[7])));
+  for (; i < n; i++) res = R::add(res, term(off + i));
+  return res;
+}
+
+template <typename T, typename F>
+__device__ T np_sum_of(const F& term, int n) {
+  if (n <= 128) return np_leaf_sum_of<T>(term, 0, n);
+  int off[32], len[32];
+  unsigned char phase[32];
+  T vals[32];
+  int sp = 1, vp = 0;
+  off[0] = 0; len[0] = n; phase[0] = 0;
+  while (sp > 0) {
+    const int top = sp - 1;
+    const int o = off[top], l = len[top];
+    if (l <= 128) {
+      vals[vp++] = np_leaf_sum_of<T>(term, o, l);
+      sp--;
+    } else {
+      int n2 = l / 2;
+      n2 -= n2 % 8;
+      if (phase[top] == 0) { phase[top] = 1; off[sp] = o; len[sp] = n2; phase[sp] = 0; sp++; }
+      else if (phase[top] == 1) { phase[top] = 2; off[sp] = o + n2; len[sp] = l - n2; phase[sp] = 0; sp++; }
+      else { const T r = vals[--vp]; const T a = vals[--vp]; vals[vp++] = Rn<T>::add(a, r); sp--; }
+    }
+  }
+  return vals[0];
+}
+
+// one leaf by a group of 8 consecutive lanes, as np_leaf_sumsq_g8
+template <typename T, typename F>
+__device__ __forceinline__ T np_leaf_sum_of_g8(const F& term, int off, int n, int sub, unsigned gmask) {
+  using R = Rn<T>;
+  if (n < 8) {
+    T res = (T)0;
+    for (int i = 0; i < n; i++) res = R::add(res, term(off + i));
+    return res;
+  }
+  const int lim = n - (n % 8);
+  T t[16];
+#pragma unroll
+  for (int u = 0; u < 16; u++) {
+    const int idx = 8 * u + sub;
+    t[u] = idx < lim ? term(off + idx) : (T)0;
+  }
+  T tail[7];
+#pragma unroll
+  for (int u = 0; u < 7; u++) tail[u] = lim + u < n ? term(off + lim + u) : (T)0;
+  T r = t[0];
+#pragma unroll
+  for (int u = 1; u < 16; u++)
+    if (8 * u < lim) r = R::add(r, t[u]);
+  r = R::add(r, __shfl_xor_sync(gmask, r, 1));
+  r = R::add(r, __shfl_xor_sync(gmask, r, 2));
+  r = R::add(r, __shfl_xor_sync(gmask, r, 4));
+#pragma unroll
+  for (int u = 0; u < 7; u++)
+    if (lim + u < n) r = R::add(r, tail[u]);
+  return r;
+}
+
 // ---- the same pairwise sum driven by a precomputed leaf program (long traces) ------------------
 // NumPy's recursion (blocks > 128 split at n/2 - (n/2)%8) visits its leaves left to right and combines
 // the partial sums as a binary tree in post-order.  For a given trace width that schedule is fixed, so the

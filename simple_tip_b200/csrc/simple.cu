@@ -1,5 +1,5 @@
 // simple.cu — bandwidth-bound kernels and small utilities of libb200tip.so:
-//   DeepGini (deepgini.py:31-35), KMNC (neuron_coverage.py:65-94), operand packing for the
+//   softmax row statistics (DeepGini deepgini.py:31-35, max softmax, PCS, softmax entropy), MC-dropout votes, KMNC (neuron_coverage.py:65-94), operand packing for the
 //   tensor-core pass, row gather, LSA whitening, LSE partial merge, and the C-ABI basics.
 #include <stdarg.h>
 #include <algorithm>
@@ -48,16 +48,38 @@ int sm_count() {
 }
 
 // =============================================================================================
-// DeepGini
+// Softmax row statistics: DeepGini, max softmax, prediction confidence score, softmax entropy
 // =============================================================================================
+// One kernel family, templated on the statistic (TIP_STAT_*): every instance shares the staging, the
+// first-index argmax and, where it sums, NumPy's pairwise order.
+//   GINI     1 - sum(p*p)                      (deepgini.py:31-35)
+//   MAX      max(p)                            (uwiz MaxSoftmax)
+//   PCS      top-1 - top-2 of p, duplicates counted (uwiz PredictionConfidenceScore: sort, s[-1] - s[-2])
+//   ENTROPY  -sum(q*log2(q)), q = p with exact zeros replaced by 1e-20 (uwiz SoftmaxEntropy)
 // Narrow rows (c <= kGiniSmallC): a block stages 128 rows in shared memory with coalesced
 // 16-byte-agnostic loads, then one thread per row walks its row in NumPy's pairwise order.
 constexpr int kGiniRows = 128;
 
+// q*log2(q) of the entropy, in T.  float32: log2 in double rounded once to float, which is what a correctly
+// rounded log2f gives (libm's is within an ulp of it); float64: CUDA's log2 (1 ulp).
+__device__ __forceinline__ float entropy_term(float p) {
+  const float q = p == 0.f ? 1e-20f : p;
+  return __fmul_rn(q, (float)log2((double)q));
+}
+__device__ __forceinline__ double entropy_term(double p) {
+  const double q = p == 0.0 ? 1e-20 : p;
+  return __dmul_rn(q, log2(q));
+}
+
 template <typename T>
-__global__ void __launch_bounds__(kGiniRows) gini_small_kernel(const T* __restrict__ p, int64_t n, int c,
-                                                               int32_t* __restrict__ pred,
-                                                               T* __restrict__ gini) {
+struct EntropyTerms {
+  const T* x;
+  __device__ __forceinline__ T operator()(int i) const { return entropy_term(x[i]); }
+};
+
+template <int STAT, typename T>
+__global__ void __launch_bounds__(kGiniRows) rowstat_small_kernel(const T* __restrict__ p, int64_t n, int c,
+                                                                  int32_t* __restrict__ pred, T* __restrict__ out) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   T* tile = reinterpret_cast<T*>(smem_raw);
   const int stride = c + 1;  // +1 padding: thread r reads tile[r*stride + k], conflict-free for odd strides
@@ -74,13 +96,23 @@ __global__ void __launch_bounds__(kGiniRows) gini_small_kernel(const T* __restri
       const T* row = tile + threadIdx.x * stride;
       int best = 0;
       T bv = row[0];
+      T second = -Rn<T>::inf();   // PCS: the largest value after bv (equal to bv when the maximum repeats)
       for (int k = 1; k < c; k++) {
         const T v = row[k];
-        if (v > bv) { bv = v; best = k; }
+        if constexpr (STAT == TIP_STAT_PCS) {
+          if (v > bv) { second = bv; bv = v; best = k; }
+          else if (v > second) second = v;
+        } else {
+          if (v > bv) { bv = v; best = k; }
+        }
       }
-      const T ss = np_sumsq<T>(row, nullptr, c);
+      T res;
+      if constexpr (STAT == TIP_STAT_GINI) res = Rn<T>::sub((T)1, np_sumsq<T>(row, nullptr, c));
+      else if constexpr (STAT == TIP_STAT_MAX) res = bv;
+      else if constexpr (STAT == TIP_STAT_PCS) res = Rn<T>::sub(bv, second);
+      else res = -np_sum_of<T>(EntropyTerms<T>{row}, c);
       pred[row0 + threadIdx.x] = best;
-      gini[row0 + threadIdx.x] = Rn<T>::sub((T)1, ss);
+      out[row0 + threadIdx.x] = res;
     }
     __syncthreads();
   }
@@ -90,7 +122,7 @@ __global__ void __launch_bounds__(kGiniRows) gini_small_kernel(const T* __restri
 // host builds it once per width: the list of <=128-element leaves and a post-order combine
 // program.  The row is staged in shared memory with coalesced loads; the four 8-lane groups of
 // the warp evaluate leaves cooperatively (lane j owns NumPy's stride-8 accumulator j), lane 0 then
-// runs the combine program over the leaf sums.
+// runs the combine program over the leaf sums.  MAX and PCS need no sum: one coalesced pass and a warp merge.
 constexpr int kGiniMaxLeaves = 1024;
 constexpr int kGiniStageElems = 4096;   // rows up to this width are staged in shared memory
 
@@ -139,10 +171,11 @@ static int gini_tree_for(int c, GiniTree* out) {
   return TIP_OK;
 }
 
-template <typename T>
-__global__ void __launch_bounds__(128) gini_wide_kernel(const T* __restrict__ p, int64_t n, int c, GiniTree tree,
-                                                        bool staged, int32_t* __restrict__ pred,
-                                                        T* __restrict__ gini) {
+template <int STAT, typename T>
+__global__ void __launch_bounds__(128) rowstat_wide_kernel(const T* __restrict__ p, int64_t n, int c, GiniTree tree,
+                                                           bool staged, int32_t* __restrict__ pred,
+                                                           T* __restrict__ out) {
+  constexpr bool kSums = STAT == TIP_STAT_GINI || STAT == TIP_STAT_ENTROPY;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int sub = lane & 7, grp = lane >> 3;
@@ -155,66 +188,196 @@ __global__ void __launch_bounds__(128) gini_wide_kernel(const T* __restrict__ p,
     // coalesced pass: argmax (first occurrence) and, if the row fits, a copy into shared memory
     T bv = src[0];
     int bi = 0;
+    T t1 = -Rn<T>::inf(), t2 = -Rn<T>::inf();   // PCS: this lane's two largest elements (a multiset)
     for (int k = lane; k < c; k += 32) {
       const T v = src[k];
-      if (staged) stage[k] = v;
+      if constexpr (kSums) {
+        if (staged) stage[k] = v;
+      }
+      if constexpr (STAT == TIP_STAT_PCS) {
+        if (v > t1) { t2 = t1; t1 = v; }
+        else if (v > t2) t2 = v;
+      }
       if (v > bv || (v == bv && k < bi)) { bv = v; bi = k; }
     }
     for (int o = 16; o > 0; o >>= 1) {
       const T ov = __shfl_xor_sync(0xffffffffu, bv, o);
       const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
       if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
-    }
-    __syncwarp();
-    const T* x = staged ? stage : src;
-    for (int l0 = 0; l0 < tree.n_leaves; l0 += 4) {
-      const int l = l0 + grp;
-      if (l < tree.n_leaves) {
-        const T s = np_leaf_sumsq_g8<T>(x + tree.leaf_off[l], nullptr, tree.leaf_len[l], sub, gmask);
-        if (sub == 0) leaf_sums[l] = s;
+      if constexpr (STAT == TIP_STAT_PCS) {
+        const T o1 = __shfl_xor_sync(0xffffffffu, t1, o), o2 = __shfl_xor_sync(0xffffffffu, t2, o);
+        t2 = max(min(t1, o1), max(t2, o2));
+        t1 = max(t1, o1);
       }
     }
-    __syncwarp();
+    if constexpr (kSums) {
+      __syncwarp();
+      const T* x = staged ? stage : src;
+      for (int l0 = 0; l0 < tree.n_leaves; l0 += 4) {
+        const int l = l0 + grp;
+        if (l < tree.n_leaves) {
+          T s;
+          if constexpr (STAT == TIP_STAT_GINI) s = np_leaf_sumsq_g8<T>(x + tree.leaf_off[l], nullptr, tree.leaf_len[l], sub, gmask);
+          else s = np_leaf_sum_of_g8<T>(EntropyTerms<T>{x}, tree.leaf_off[l], tree.leaf_len[l], sub, gmask);
+          if (sub == 0) leaf_sums[l] = s;
+        }
+      }
+      __syncwarp();
+    }
     if (lane == 0) {
-      T stack[32];
-      int sp = 0;
-      for (int i = 0; i < tree.n_prog; i++) {
-        const int op = tree.prog[i];
-        if (op >= 0) stack[sp++] = leaf_sums[op];
-        else { const T r = stack[--sp]; const T a = stack[--sp]; stack[sp++] = Rn<T>::add(a, r); }
+      T res;
+      if constexpr (kSums) {
+        T stack[32];
+        int sp = 0;
+        for (int i = 0; i < tree.n_prog; i++) {
+          const int op = tree.prog[i];
+          if (op >= 0) stack[sp++] = leaf_sums[op];
+          else { const T r = stack[--sp]; const T a = stack[--sp]; stack[sp++] = Rn<T>::add(a, r); }
+        }
+        if constexpr (STAT == TIP_STAT_GINI) res = Rn<T>::sub((T)1, stack[0]);
+        else res = -stack[0];
+      } else if constexpr (STAT == TIP_STAT_MAX) {
+        res = bv;
+      } else {
+        res = Rn<T>::sub(t1, t2);
       }
       pred[row] = bi;
-      gini[row] = Rn<T>::sub((T)1, stack[0]);
+      out[row] = res;
     }
     __syncwarp();
   }
 }
 
-template <typename T>
-static int launch_gini(const T* p, int64_t n, int64_t c, int32_t* pred, T* gini, cudaStream_t st) {
+template <int STAT, typename T>
+static int launch_rowstat(const T* p, int64_t n, int64_t c, int32_t* pred, T* out, cudaStream_t st) {
+  constexpr bool kSums = STAT == TIP_STAT_GINI || STAT == TIP_STAT_ENTROPY;
   const int sms = sm_count();
   const size_t small_bytes = (size_t)kGiniRows * (size_t)(c + 1) * sizeof(T);
   if (small_bytes <= 96 * 1024) {
-    TIP_CHECK_CUDA(cudaFuncSetAttribute(gini_small_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    TIP_CHECK_CUDA(cudaFuncSetAttribute(rowstat_small_kernel<STAT, T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                         (int)small_bytes));
     const int64_t blocks = (n + kGiniRows - 1) / kGiniRows;
     const int grid = (int)std::min<int64_t>(blocks, (int64_t)sms * 8);
-    gini_small_kernel<T><<<grid, kGiniRows, small_bytes, st>>>(p, n, (int)c, pred, gini);
+    rowstat_small_kernel<STAT, T><<<grid, kGiniRows, small_bytes, st>>>(p, n, (int)c, pred, out);
   } else {
-    TIP_REQUIRE(c <= (int64_t)kGiniMaxLeaves * 64, "row too wide");
     GiniTree tree;
-    int rc = gini_tree_for((int)c, &tree);
-    if (rc != TIP_OK) return rc;
-    TIP_REQUIRE(tree.n_leaves <= kGiniMaxLeaves, "row too wide");
-    const bool staged = c <= kGiniStageElems;
-    const size_t bytes = 4 * (size_t)tree.n_leaves * sizeof(T) + (staged ? 4 * (size_t)c * sizeof(T) : 0);
-    TIP_CHECK_CUDA(cudaFuncSetAttribute(gini_wide_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        (int)(4 * (kGiniMaxLeaves + kGiniStageElems) * sizeof(T))));
+    bool staged = false;
+    size_t bytes = 0;
+    if (kSums) {
+      TIP_REQUIRE(c <= (int64_t)kGiniMaxLeaves * 64, "row too wide");
+      int rc = gini_tree_for((int)c, &tree);
+      if (rc != TIP_OK) return rc;
+      TIP_REQUIRE(tree.n_leaves <= kGiniMaxLeaves, "row too wide");
+      staged = c <= kGiniStageElems;
+      bytes = 4 * (size_t)tree.n_leaves * sizeof(T) + (staged ? 4 * (size_t)c * sizeof(T) : 0);
+      TIP_CHECK_CUDA(cudaFuncSetAttribute(rowstat_wide_kernel<STAT, T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                          (int)(4 * (kGiniMaxLeaves + kGiniStageElems) * sizeof(T))));
+    }
     const int grid = (int)std::min<int64_t>((n + 3) / 4, (int64_t)sms * 16);
-    gini_wide_kernel<T><<<grid, 128, bytes, st>>>(p, n, (int)c, tree, staged, pred, gini);
+    rowstat_wide_kernel<STAT, T><<<grid, 128, bytes, st>>>(p, n, (int)c, tree, staged, pred, out);
   }
   TIP_LAUNCH_CHECK();
   return TIP_OK;
+}
+
+template <typename T>
+static int launch_softmax_stat(const T* p, int64_t n, int64_t c, int kind, int32_t* pred, T* out, cudaStream_t st) {
+  switch (kind) {
+    case TIP_STAT_GINI: return launch_rowstat<TIP_STAT_GINI, T>(p, n, c, pred, out, st);
+    case TIP_STAT_MAX: return launch_rowstat<TIP_STAT_MAX, T>(p, n, c, pred, out, st);
+    case TIP_STAT_PCS: return launch_rowstat<TIP_STAT_PCS, T>(p, n, c, pred, out, st);
+    case TIP_STAT_ENTROPY: return launch_rowstat<TIP_STAT_ENTROPY, T>(p, n, c, pred, out, st);
+  }
+  TIP_REQUIRE(false, "kind must be one of TIP_STAT_*");
+}
+
+// =============================================================================================
+// Votes of sampled predictions (uwiz VariationRatio over MC-dropout samples)
+// =============================================================================================
+// Sample s of row i is the c-vector at probs + i * row_stride + s * sample_stride.  A block owns kVoteRows
+// consecutive rows (enough that it has ~256 sampled rows to reduce) and counts their votes in shared memory, then adds
+// the counts to the caller's running [n, c] tally (the same rows belong to the same block of every launch on the
+// stream, so no global atomics).  Narrow rows: one thread per sampled row; wider ones: one warp per sampled row.
+constexpr int kVoteThreads = 256;
+constexpr int kVoteThreadC = 32;          // up to this width a sampled row is one thread's serial argmax
+constexpr int kVoteSmemInts = 12 * 1024;  // 48 KB of shared counts per block; wider rows count in global memory
+
+template <typename T>
+__global__ void __launch_bounds__(kVoteThreads) vote_add_kernel(const T* __restrict__ p, int64_t n, int c,
+                                                                int samples, int64_t sample_stride,
+                                                                int64_t row_stride, int rows_per_block,
+                                                                int32_t* __restrict__ counts) {
+  extern __shared__ int vote_smem[];
+  const int64_t i0 = (int64_t)blockIdx.x * rows_per_block;
+  const int rows = (int)min((int64_t)rows_per_block, n - i0);
+  const bool shared_hist = rows_per_block * c <= kVoteSmemInts;
+  int* hist = shared_hist ? vote_smem : counts + i0 * c;
+  if (shared_hist) {
+    for (int j = threadIdx.x; j < rows * c; j += kVoteThreads) vote_smem[j] = 0;
+    __syncthreads();
+  }
+  const int items = rows * samples;
+  if (c <= kVoteThreadC) {
+    for (int m = threadIdx.x; m < items; m += kVoteThreads) {
+      const int r = m / samples, s = m - r * samples;
+      const T* x = p + (i0 + r) * row_stride + (int64_t)s * sample_stride;
+      T bv = x[0];
+      int best = 0;
+      for (int k = 1; k < c; k++) {
+        const T v = x[k];
+        if (v > bv) { bv = v; best = k; }
+      }
+      atomicAdd(hist + r * c + best, 1);
+    }
+  } else {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int m = warp; m < items; m += kVoteThreads / 32) {
+      const int r = m / samples, s = m - r * samples;
+      const T* x = p + (i0 + r) * row_stride + (int64_t)s * sample_stride;
+      T bv = x[0];
+      int bi = 0;
+      for (int k = lane; k < c; k += 32) {
+        const T v = x[k];
+        if (v > bv || (v == bv && k < bi)) { bv = v; bi = k; }
+      }
+      for (int o = 16; o > 0; o >>= 1) {
+        const T ov = __shfl_xor_sync(0xffffffffu, bv, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+        if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+      }
+      if (lane == 0) atomicAdd(hist + r * c + bi, 1);
+    }
+  }
+  if (shared_hist) {
+    __syncthreads();
+    int32_t* dst = counts + i0 * c;
+    for (int j = threadIdx.x; j < rows * c; j += kVoteThreads)
+      if (vote_smem[j]) dst[j] += vote_smem[j];
+  }
+}
+
+// pred[i] = the lowest class with the most votes (scipy.stats.mode), vr[i] = 1 - votes / samples in float64
+__global__ void __launch_bounds__(256) vote_finish_kernel(const int32_t* __restrict__ counts, int64_t n, int c,
+                                                          int samples, int32_t* __restrict__ pred,
+                                                          double* __restrict__ vr) {
+  const int lane = threadIdx.x & 31;
+  const int64_t row = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (row >= n) return;
+  const int32_t* h = counts + row * c;
+  int bv = -1, bi = 0;
+  for (int k = lane; k < c; k += 32) {
+    const int v = h[k];
+    if (v > bv) { bv = v; bi = k; }
+  }
+  for (int o = 16; o > 0; o >>= 1) {
+    const int ov = __shfl_xor_sync(0xffffffffu, bv, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+    if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+  }
+  if (lane == 0) {
+    pred[row] = bi;
+    vr[row] = __dsub_rn(1.0, __ddiv_rn((double)bv, (double)samples));
+  }
 }
 
 // =============================================================================================
@@ -829,10 +992,52 @@ extern "C" int tip_deepgini(const void* probs, int dtype, int64_t n, int64_t c, 
   TIP_REQUIRE(probs && pred && gini, "null pointer");
   TIP_REQUIRE(n >= 0 && c >= 1 && c < (1 << 30), "shape");
   if (n == 0) return TIP_OK;
+  return tip_softmax_stat(probs, dtype, n, c, TIP_STAT_GINI, pred, gini, stream);
+}
+
+extern "C" int tip_softmax_stat(const void* probs, int dtype, int64_t n, int64_t c, int kind, int32_t* pred,
+                                void* out, void* stream) {
+  TIP_REQUIRE(n >= 0 && c >= 1 && c < (1 << 30), "shape");
+  TIP_REQUIRE(kind != TIP_STAT_PCS || c >= 2, "PCS needs at least two classes");
+  if (n == 0) return TIP_OK;   // (empty buffers may come as null pointers)
+  TIP_REQUIRE(probs && pred && out, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == TIP_F32) return launch_gini<float>((const float*)probs, n, c, pred, (float*)gini, st);
-  if (dtype == TIP_F64) return launch_gini<double>((const double*)probs, n, c, pred, (double*)gini, st);
+  if (dtype == TIP_F32) return launch_softmax_stat<float>((const float*)probs, n, c, kind, pred, (float*)out, st);
+  if (dtype == TIP_F64) return launch_softmax_stat<double>((const double*)probs, n, c, kind, pred, (double*)out, st);
   TIP_REQUIRE(false, "dtype must be TIP_F32 or TIP_F64");
+}
+
+extern "C" int tip_vote_add(const void* probs, int dtype, int64_t n, int64_t c, int64_t samples, int64_t sample_stride,
+                            int64_t row_stride, int32_t* counts, void* stream) {
+  TIP_REQUIRE(n >= 0 && c >= 1 && c < (1 << 30) && samples >= 0 && samples < (1 << 30), "shape");
+  TIP_REQUIRE(sample_stride >= 0 && row_stride >= 0, "strides");
+  if (n == 0 || samples == 0) return TIP_OK;
+  TIP_REQUIRE(probs && counts, "null pointer");
+  const int rows_per_block = (int)std::max<int64_t>(1, std::min<int64_t>(kVoteThreads / samples, kVoteSmemInts / c));
+  const int64_t blocks = (n + rows_per_block - 1) / rows_per_block;
+  TIP_REQUIRE(blocks < (1LL << 31) && (int64_t)rows_per_block * samples < (1LL << 31), "too many rows");
+  const size_t smem = (int64_t)rows_per_block * c <= kVoteSmemInts ? (size_t)rows_per_block * c * sizeof(int) : 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (dtype == TIP_F32)
+    vote_add_kernel<float><<<(unsigned)blocks, kVoteThreads, smem, st>>>((const float*)probs, n, (int)c, (int)samples,
+                                                                          sample_stride, row_stride, rows_per_block, counts);
+  else if (dtype == TIP_F64)
+    vote_add_kernel<double><<<(unsigned)blocks, kVoteThreads, smem, st>>>((const double*)probs, n, (int)c, (int)samples,
+                                                                           sample_stride, row_stride, rows_per_block, counts);
+  else
+    TIP_REQUIRE(false, "dtype must be TIP_F32 or TIP_F64");
+  TIP_LAUNCH_CHECK();
+  return TIP_OK;
+}
+
+extern "C" int tip_vote_finish(const int32_t* counts, int64_t n, int64_t c, int64_t samples, int32_t* pred, double* vr,
+                               void* stream) {
+  TIP_REQUIRE(n >= 0 && c >= 1 && c < (1 << 30) && samples >= 1, "shape");
+  if (n == 0) return TIP_OK;
+  TIP_REQUIRE(counts && pred && vr, "null pointer");
+  vote_finish_kernel<<<(unsigned)((n + 7) / 8), 256, 0, (cudaStream_t)stream>>>(counts, n, (int)c, (int)samples, pred, vr);
+  TIP_LAUNCH_CHECK();
+  return TIP_OK;
 }
 
 extern "C" int tip_kmnc(const void* act, int act_dtype, int64_t n, int64_t d, const void* mins, const void* jumps,
