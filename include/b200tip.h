@@ -161,6 +161,18 @@ int tip_cam_buckets(const void* bucket, int bucket_dtype, int64_t n, int64_t d, 
                     int32_t* gain, uint32_t* covered, int32_t* newlist, int32_t* order, int32_t* state,
                     int32_t rounds, void* stream);
 
+/* ---- Surprise-coverage CAM (handler_surprise.py:101-115, prioritizers.py:16-45) ---------------------
+ * The greedy picks of cam(values, SurpriseCoverageMapper.get_coverage_profile(values)) without the n x sections
+ * profile.  thresholds: sections + 1 float64 values on the device, NaN-free and non-decreasing (the caller checks;
+ * then every profile row has at most one True and the picks are the first sample of every non-empty bucket, in
+ * ascending sample order).  values: n values of TIP_F32 (compared after exact widening to float64, NumPy's
+ * promotion) or TIP_F64; sample i lies in bucket b when thresholds[b] <= v < thresholds[b+1]; NaN lies in none.
+ * first[sections] uint32 scratch (reset here); out: order[0..count) = the picks, count[1] int32.
+ * 1 <= sections <= TIP_SC_CAM_MAX_SECTIONS (one block ranks the buckets in shared memory), 0 <= n < 2^31. */
+#define TIP_SC_CAM_MAX_SECTIONS 4096
+int tip_sc_cam(const void* values, int dtype, int64_t n, const double* thresholds, int32_t sections,
+               uint32_t* first, int32_t* order, int32_t* count, void* stream);
+
 /* ---- sibling coverage criteria and their fit step (neuron_coverage.py:52-62,97-173;
  * aggregate_statistics.py:37-67 + welford==0.2.5) ------------------------------------------
  * tip_cover_threshold: act n x d (TIP_F32/TIP_F64); mode

@@ -16,6 +16,7 @@ LIB_PATH = os.path.join(_HERE, "libb200tip.so")
 TIP_F32, TIP_F64, TIP_BF16, TIP_I16, TIP_I32 = 0, 1, 2, 3, 4
 COVER_NAC, COVER_SNAC, COVER_NBC = 0, 1, 2
 CAM_MAX_BLOCKS = 1024
+SC_CAM_MAX_SECTIONS = 4096      # TIP_SC_CAM_MAX_SECTIONS
 ROLE_QUERY, ROLE_TRAIN = 0, 1
 RANGE_SAME_CLASS, RANGE_OTHER_CLASSES = 0, 1
 ROW_TILE, COL_TILE = 128, 256
@@ -49,6 +50,7 @@ _SIGNATURES = {
     "tip_vote_finish": (C.c_int, [_vp, _i64, _i64, _i64, _vp, _vp, _vp]),
     "tip_kmnc": (C.c_int, [_vp, C.c_int, _i64, _i64, _vp, _vp, C.c_int, _i32, _vp, C.c_int, _vp, _vp]),
     "tip_cam_buckets": (C.c_int, [_vp, C.c_int, _i64, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _vp]),
+    "tip_sc_cam": (C.c_int, [_vp, C.c_int, _i64, _vp, _i32, _vp, _vp, _vp, _vp]),
     "tip_cover_packed_words": (_i64, [_i64]),
     "tip_cover_threshold": (C.c_int, [_vp, C.c_int, _i64, _i64, _vp, _vp, C.c_int, C.c_double, C.c_int, _vp, _vp, _vp, _vp]),
     "tip_tknc": (C.c_int, [_vp, C.c_int, _i64, _i64, _i32, _vp, _i64, _i64, _vp, _i64, _vp]),

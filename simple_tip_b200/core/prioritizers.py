@@ -4,7 +4,8 @@
 profile (`cam_from_bits`, one persistent cooperative kernel), which is also the entry point for profiles that
 never left HBM (`NAC/NBC/SNAC/TKNC.packed`).  `cam_from_buckets` is the same ordering for k-multisection profiles given in their compact form
 (the bucket ids of `KMNC.buckets`): the greedy loop runs on the GPU (libb200tip `tip_cam_buckets`)
-without ever building the N x D x k array, which is 41 GB at k = 1000."""
+without ever building the N x D x k array, which is 41 GB at k = 1000.  `cam_from_surprise` is the ordering for
+surprise-coverage profiles (`SurpriseCoverageMapper`): one pass over the scores (libb200tip `tip_sc_cam`)."""
 from typing import Generator
 
 import numpy as np
@@ -157,3 +158,54 @@ def cam_from_buckets(scores: np.ndarray, bucket, sections: int) -> Generator[int
     LAST_GREEDY_PICKS = int(greedy.shape[0])
     yield from (int(i) for i in greedy)
     yield from _tail_by_score(scores, greedy)
+
+
+def thresholds_one_hot(thresholds: np.ndarray) -> bool:
+    """True when the bucket edges are NaN-free and non-decreasing, so that the buckets [t[b], t[b+1]) are disjoint
+    and every row of `SurpriseCoverageMapper.get_coverage_profile` holds at most one True.  np.linspace breaks this
+    for a negative, NaN or +inf upper bound (+inf is what np.max picks up from LSA scores whose density underflowed)."""
+    t = np.asarray(thresholds, dtype=np.float64)
+    return not np.isnan(t).any() and bool(np.all(t[1:] >= t[:-1]))
+
+
+def cam_from_surprise(scores, mapper) -> Generator[int, None, None]:
+    """`cam(scores, mapper.get_coverage_profile(scores))` for a `SurpriseCoverageMapper` (handler_surprise.py:101-115),
+    without the N x sections profile.  scores: float32 or float64, NumPy or a CUDA tensor.
+
+    When the mapper's thresholds pass `thresholds_one_hot`, the profile is one-hot, and the reference's greedy loop
+    picks the first sample of every non-empty bucket in ascending sample order: one pass over the scores on the GPU
+    (libb200tip `tip_sc_cam`) finds them.  Otherwise the dense profile is built with the mapper's own expression and
+    ordered by `cam`.  The rest follows by `np.argsort(-scores)` on the host in the scores' own dtype, so ties fall
+    as in the reference.  At most `_lib.SC_CAM_MAX_SECTIONS` sections (ValueError before any launch)."""
+    import torch
+
+    from .. import _lib
+    from .. import engine as E
+
+    thresholds = np.asarray(mapper.thresholds, dtype=np.float64)
+    sections = thresholds.shape[0] - 1
+    if not 1 <= sections <= _lib.SC_CAM_MAX_SECTIONS:
+        raise ValueError(f"cam_from_surprise takes 1 to {_lib.SC_CAM_MAX_SECTIONS} sections, got {sections}")
+    on_device = isinstance(scores, torch.Tensor)
+    host = scores.detach().cpu().numpy() if on_device else np.asarray(scores)
+    assert host.ndim == 1
+    dtype = E.tip_dtype(host.dtype)
+    if not thresholds_one_hot(thresholds):
+        yield from cam(host, mapper.get_coverage_profile(host))
+        return
+    n = host.shape[0]
+    greedy = np.zeros(0, dtype=np.int64)
+    if n > 0:
+        dev = E.require_cuda()
+        values = scores.detach().to(dev).contiguous() if on_device else torch.from_numpy(np.ascontiguousarray(host)).to(dev)
+        t = torch.from_numpy(thresholds).to(dev)
+        first = torch.empty(sections, dtype=torch.int32, device=dev)
+        out = torch.empty(sections + 1, dtype=torch.int32, device=dev)          # [count, order...]: one download
+        _lib.check(_lib.load().tip_sc_cam(E._p(values), dtype, n, E._p(t), sections, E._p(first), E._p(out[1:]),
+                                          E._p(out), E._stream()), "tip_sc_cam")
+        res = out.cpu().numpy()
+        greedy = res[1:1 + int(res[0])].astype(np.int64)
+    global LAST_GREEDY_PICKS
+    LAST_GREEDY_PICKS = int(greedy.shape[0])
+    yield from (int(i) for i in greedy)
+    yield from _tail_by_score(host.copy(), greedy)

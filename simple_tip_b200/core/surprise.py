@@ -132,11 +132,19 @@ def _trace_matrix(activations):
     return x if x is not None else _flatten_layers(activations)
 
 
+def _host_matrix(activations) -> np.ndarray:
+    """[N, D] host traces: torch CUDA traces downloaded once, else the reference's host flattening."""
+    from .. import engine as E
+
+    x = E.device_matrix(activations)
+    return x.cpu().numpy() if x is not None else _flatten_layers(activations)
+
+
 class _KmeansDiscriminator:
     """k-means modal assignment with silhouette model selection (surprise.py:102-133).
-    backend="sklearn" (default): sklearn on the host, as the reference.  backend="device": k-means and the
-    silhouette score on the GPU (core/clustering.py), seeded with `random_state` (the reference's sklearn call
-    is unseeded); the traces may then be torch CUDA tensors."""
+    backend="sklearn" (default): sklearn on the host, as the reference; torch CUDA traces are downloaded once per
+    call.  backend="device": k-means and the silhouette score on the GPU (core/clustering.py), seeded with
+    `random_state` (the reference's sklearn call is unseeded); CUDA traces stay on the device."""
 
     def __init__(self, training_data: Activations, potential_k: Iterable[int], subsampling=1.0,
                  subsampling_seed: int = 0, n_init: int = 10, max_iter: int = 300, backend: Optional[str] = None,
@@ -152,7 +160,7 @@ class _KmeansDiscriminator:
             from sklearn.cluster import KMeans
             from sklearn.metrics import silhouette_score
 
-            data = _subsample_array(subsampling, _flatten_layers(training_data), seed=subsampling_seed)
+            data = _subsample_array(subsampling, _host_matrix(training_data), seed=subsampling_seed)
         self.best_score, self.best_k, self.best_clusterer = -np.inf, None, None
         for k in potential_k:
             if self.backend == "device":
@@ -168,7 +176,7 @@ class _KmeansDiscriminator:
             from .. import engine as E
 
             return E.host_array(self.best_clusterer.predict(_trace_matrix(activations)))
-        return self.best_clusterer.predict(_flatten_layers(activations))
+        return self.best_clusterer.predict(_host_matrix(activations))
 
 
 class SurpriseCoverageMapper:
@@ -235,12 +243,7 @@ class MultiModalSA(SA):
                                     subsampling=subsampling, subsampling_seed=subsampling_seed, backend=backend,
                                     random_state=random_state)
         if disc.backend == "device":
-            # the modal SAs are fitted on host rows, as the reference does
-            from .. import engine as E
-
-            x = E.device_matrix(activations)
-            if x is not None:
-                activations = x.cpu().numpy()
+            activations = _host_matrix(activations)      # the modal SAs are fitted on host rows, as the reference does
         return MultiModalSA.build(activations, predictions, disc, sa_constructor)
 
     @staticmethod
@@ -274,9 +277,13 @@ class MultiModalSA(SA):
             raise ValueError(f"No modal found for modal id {modal_id}. Check your discriminator")
 
     def __call__(self, activations, predictions, num_threads: int = 1) -> np.ndarray:
+        """CUDA traces (one tensor or a list of hook layers) are split by modal on the device, whatever the
+        discriminator; NumPy traces are flattened on the host, as the reference does."""
+        from .. import engine as E
+
+        predictions = E.host_array(predictions)
         modal = self.discriminator(activations, predictions)
-        on_device = isinstance(self.discriminator, _KmeansDiscriminator) and self.discriminator.backend == "device"
-        acts = _trace_matrix(activations) if on_device else _flatten_layers(activations)
+        acts = _trace_matrix(activations)
         preds = _flatten_predictions(predictions)
         assert len(modal) == acts.shape[0], (
             f"The discriminator returned an invalid number ({len(modal)}) of modal indexes."
@@ -372,8 +379,7 @@ class MDSA(SA):
         else:
             from sklearn.covariance import EmpiricalCovariance
 
-            host = E.device_matrix(activations)
-            acts = host.cpu().numpy() if host is not None else _flatten_layers(activations)
+            acts = _host_matrix(activations)
         self.covariance_matrix = EmpiricalCovariance()
         self.covariance_matrix.fit(acts)
         self._width = int(acts.shape[1])
@@ -427,8 +433,7 @@ class MLSA(SA):
         else:
             from sklearn.mixture import GaussianMixture
 
-            host = E.device_matrix(activations)
-            acts = host.cpu().numpy() if host is not None else _flatten_layers(activations)
+            acts = _host_matrix(activations)
             self.gmm = GaussianMixture(n_components=num_components)
         self.gmm.fit(acts)
         self._width = int(acts.shape[1])

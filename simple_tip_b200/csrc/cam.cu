@@ -106,6 +106,77 @@ static int launch_cam(const void* bucket, int64_t n, int64_t d, int32_t k, int32
   return TIP_OK;
 }
 
+// ---- Surprise-coverage CAM (handler_surprise.py:101-115 over prioritizers.py:16-45) -------------------------
+// SurpriseCoverageMapper's profile is profile[i, b] = t[b] <= v[i] < t[b+1].  For NaN-free, non-decreasing t the
+// buckets are disjoint, so every row holds at most one True: a sample's gain is 1 while its bucket is uncovered
+// and 0 after, np.argmax takes the lowest such index, and covering a bucket zeroes every other sample in it.  The
+// greedy picks are therefore the first sample of every non-empty bucket, in ascending sample order.  One pass
+// finds each bucket's first sample (sc_first_kernel); one block sorts those (sc_rank_kernel).
+constexpr int kScThreads = 256;
+constexpr uint32_t kScNone = 0xffffffffu;      // bucket without a sample; larger than every index
+
+template <typename T>
+__global__ void __launch_bounds__(kScThreads) sc_first_kernel(const T* __restrict__ v, int n,
+                                                              const double* __restrict__ t, int sections,
+                                                              uint32_t* __restrict__ first) {
+  extern __shared__ double s_t[];                        // t[0..sections], then the block's first[0..sections)
+  uint32_t* s_first = reinterpret_cast<uint32_t*>(s_t + sections + 1);
+  for (int j = threadIdx.x; j <= sections; j += kScThreads) s_t[j] = t[j];
+  for (int j = threadIdx.x; j < sections; j += kScThreads) s_first[j] = kScNone;
+  __syncthreads();
+  for (int i = blockIdx.x * kScThreads + threadIdx.x; i < n; i += gridDim.x * kScThreads) {
+    const double x = (double)v[i];                       // float32 -> float64 is exact: NumPy's promotion
+    int lo = 0, hi = sections + 1;                       // lo = number of thresholds <= x (NaN: 0)
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (s_t[mid] <= x) lo = mid + 1; else hi = mid;
+    }
+    const int b = lo - 1;
+    if (b >= 0 && b < sections && s_t[b] <= x && x < s_t[b + 1] && (uint32_t)i < s_first[b])
+      atomicMin(s_first + b, (uint32_t)i);
+  }
+  __syncthreads();
+  for (int j = threadIdx.x; j < sections; j += kScThreads)
+    if (s_first[j] != kScNone) atomicMin(first + j, s_first[j]);
+}
+
+// order[rank] = first[b] for every non-empty bucket, rank = number of smaller entries (the entries are distinct
+// sample indices); count = number of non-empty buckets.
+__global__ void __launch_bounds__(1024) sc_rank_kernel(const uint32_t* __restrict__ first, int sections,
+                                                       int32_t* __restrict__ order, int32_t* __restrict__ count) {
+  __shared__ uint32_t s_f[TIP_SC_CAM_MAX_SECTIONS];
+  __shared__ int s_count;
+  if (threadIdx.x == 0) s_count = 0;
+  for (int j = threadIdx.x; j < sections; j += 1024) s_f[j] = first[j];
+  __syncthreads();
+  int mine = 0;
+  for (int j = threadIdx.x; j < sections; j += 1024) {
+    const uint32_t f = s_f[j];
+    if (f == kScNone) continue;
+    int rank = 0;
+    for (int k = 0; k < sections; k++) rank += s_f[k] < f;
+    order[rank] = (int32_t)f;
+    mine++;
+  }
+  mine = warp_sum(mine);
+  if ((threadIdx.x & 31) == 0 && mine) atomicAdd(&s_count, mine);
+  __syncthreads();
+  if (threadIdx.x == 0) *count = s_count;
+}
+
+template <typename T>
+static int launch_sc_first(const void* values, int64_t n, const double* t, int sections, uint32_t* first,
+                           cudaStream_t st) {
+  const size_t smem = (size_t)(sections + 1) * sizeof(double) + (size_t)sections * sizeof(uint32_t);
+  if (smem > 48 * 1024)
+    TIP_CHECK_CUDA(cudaFuncSetAttribute(sc_first_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((n + 8 * kScThreads - 1) / (8 * kScThreads),
+                                                                (int64_t)sm_count() * 4));
+  sc_first_kernel<T><<<grid, kScThreads, smem, st>>>((const T*)values, (int)n, t, sections, first);
+  TIP_LAUNCH_CHECK();
+  return TIP_OK;
+}
+
 }  // namespace tip
 
 using namespace tip;
@@ -121,4 +192,22 @@ extern "C" int tip_cam_buckets(const void* bucket, int bucket_dtype, int64_t n, 
   if (bucket_dtype == TIP_I16)
     return launch_cam<int16_t>(bucket, n, d, sections, gain, covered, newlist, order, state, rounds, st);
   return launch_cam<int32_t>(bucket, n, d, sections, gain, covered, newlist, order, state, rounds, st);
+}
+
+extern "C" int tip_sc_cam(const void* values, int dtype, int64_t n, const double* thresholds, int32_t sections,
+                          uint32_t* first, int32_t* order, int32_t* count, void* stream) {
+  TIP_REQUIRE((values || n == 0) && thresholds && first && order && count, "null pointer");
+  TIP_REQUIRE(n >= 0 && n < (1LL << 31), "shape");
+  TIP_REQUIRE(sections >= 1 && sections <= TIP_SC_CAM_MAX_SECTIONS, "sections must be in [1, TIP_SC_CAM_MAX_SECTIONS]");
+  TIP_REQUIRE(dtype == TIP_F32 || dtype == TIP_F64, "dtype must be TIP_F32 or TIP_F64");
+  cudaStream_t st = (cudaStream_t)stream;
+  TIP_CHECK_CUDA(cudaMemsetAsync(first, 0xff, (size_t)sections * sizeof(uint32_t), st));
+  if (n > 0) {
+    const int rc = dtype == TIP_F32 ? launch_sc_first<float>(values, n, thresholds, sections, first, st)
+                                    : launch_sc_first<double>(values, n, thresholds, sections, first, st);
+    if (rc != TIP_OK) return rc;
+  }
+  sc_rank_kernel<<<1, 1024, 0, st>>>(first, sections, order, count);
+  TIP_LAUNCH_CHECK();
+  return TIP_OK;
 }
