@@ -277,12 +277,12 @@ int tip_nn_filter(const void* q_pack, const float* q_sqnorm, int64_t m, const vo
                   void* stream);
 
 /* Tile geometry tip_nn_filter uses for traces of width d: work items must start on query rows
- * that are multiples of nothing in particular but cover at most *q_rows rows (128); *t_rows
- * is the train-tile height (128), useful for sizing spans. */
+ * that are multiples of nothing in particular but cover at most *q_rows rows (192 for the resident-query
+ * kernel, 128 for the streaming one); *t_rows is the train-tile height (128), useful for sizing spans. */
 int tip_nn_filter_tile(int64_t d, int32_t* q_rows, int32_t* t_rows);
 /* which tensor-core kernel tip_nn_filter runs for traces of width d: 1 = resident-query (d <= 128: the query
- * tile is loaded once per work item), 0 = streaming (query and train chunks through one ring); both use
- * 128 x 128 tiles.  tip_kde_tile_rows: query rows per work item of tip_kde_lse*. */
+ * tile is loaded once per work item; 192 x 128 tiles), 0 = streaming (query and train chunks through one
+ * ring; 128 x 128 tiles).  tip_kde_tile_rows: query rows per work item of tip_kde_lse*. */
 int tip_nn_filter_kind(int64_t d);
 int tip_kde_tile_rows(void);
 int tip_kde_slot_parts(void);   /* partial (max, sum) pairs per work-item slot: part_max / part_sum hold slots x this x m */

@@ -12,13 +12,16 @@
 //             silhouette_samples); the query's own column contributes 0
 //   MODE_DUMP raw accumulator tile (bring-up / validation)
 //
-// Roles (384 threads): warpgroup 0 = TMA producer and work-item hand-out (one lane of warp 0) and, in
-// the resident MODE_NN kernel, three drain warps; warpgroups 1 and 2 = consumers.  Consumer warpgroup g owns query rows
-// [64 g, 64 g + 64) of the tile: it issues m64n128k16 wgmma for them, keeps the accumulator in
-// registers and reduces it there.  In the wgmma accumulator layout the four lanes of a quad hold one
-// row between them (8 of every 32 consecutive columns each), so the per-row reductions finish with two
-// quad shuffles.  The two consumer warpgroups drift out of phase, so one's MMAs overlap the other's
-// reduction.
+// Roles: warpgroup 0 = TMA producer and work-item hand-out (one lane of warp 0) and, in the resident MODE_NN kernel,
+// three drain warps; warpgroups 1.. = consumers.  Consumer warpgroup g owns query rows [64 g, 64 g + 64) of the tile:
+// it issues m64n128k16 wgmma for them, keeps the accumulator in registers and reduces it there.  In the wgmma
+// accumulator layout the four lanes of a quad hold one row between them (8 of every 32 consecutive columns each), so
+// the per-row reductions finish with two quad shuffles.  The consumer warpgroups drift out of phase, so one's MMAs
+// overlap another's reduction.  The resident MODE_NN kernel has three consumer warpgroups on 192-row query tiles
+// (512 threads; warpgroup 0 hands registers to the consumers with setmaxnreg): while one reduces, the other two
+// keep the tensor core busy, and each train tile fetched from L2 feeds 1.5x the MMAs.  A consumer warpgroup whose
+// rows all lie past the item's query rows issues no MMAs.  Every other instantiation has two consumer warpgroups on
+// 128-row tiles (384 threads).
 // Pipeline: kStages-deep shared-memory ring (full/empty mbarriers, TMA -> wgmma).  Streaming variant:
 // one commit group per K chunk, each waited for and its stage released before the next chunk.
 // Resident-query variant (RESA, short packed rows): the query tile's K chunks are loaded once per run
@@ -41,7 +44,7 @@
 
 namespace tip {
 
-constexpr int BM = 128;
+constexpr int BM = 128;  // query rows per tile, except in the resident MODE_NN kernel (Layout::kRows)
 constexpr int BN = 128;
 constexpr int BK = 64;  // bf16 elements per smem row = one 128-byte swizzle atom
 constexpr int kStages = 6;
@@ -50,31 +53,42 @@ constexpr int kBBytes = BN * BK * 2;
 constexpr int kStageBytes = kABytes + kBBytes;
 constexpr int kRingBytes = kStages * kStageBytes;
 constexpr int kResAChunks = 5;               // resident-query variant: query tiles of up to 5 x 64 K elements
-constexpr int kConsumerWarps = 8;            // two consumer warpgroups
-constexpr int kThreads = 128 + 32 * kConsumerWarps;
 constexpr int kCandSlots = 8;   // per-query staging slots for candidates (MODE_NN)
-constexpr int kCandBytes = kCandSlots * BM * 12;   // value, chunk start, 32-bit column mask
 constexpr int kEvSlots = BN / 32;   // MODE_NN events per row and tile: one per 32-column chunk
 constexpr int kDrainWarps = 3;      // warps 1..3 of warpgroup 0
 // MODE_NN event mailbox, one per tile parity: the consumers record a tile's events, the drain warps stage them
 struct EvRecord { int col; uint32_t mask; float mn, thr; };   // chunk start, column mask, chunk minimum, row thr
 struct EvRow { float thr; int ev; };                          // row thr after the tile, bit c = event in chunk c
+template <int ROWS>
 struct EvBuf {
-  EvRecord rec[BM * kEvSlots];
-  EvRow row[BM];
+  EvRecord rec[ROWS * kEvSlots];
+  EvRow row[ROWS];
   int q_row0, flags, pad[2];
 };
 enum { kEvLast = 1, kEvStop = 2 };   // EvBuf::flags: last tile of the item (flush), no more tiles
-constexpr int kEvBytes = 2 * (int)sizeof(EvBuf);
 constexpr int kBarBytes = 256;
-constexpr int kSmemBytes = kRingBytes + 1024 /*align slack*/ + kBarBytes + kCandBytes + kEvBytes;
 constexpr int kSmemMax = 232448;   // 227 KB per block on sm_90
-static_assert(kResAChunks * kABytes + kStages * kBBytes <= kRingBytes, "resident-query layout does not fit");
-static_assert(kSmemBytes <= kSmemMax, "pair kernel does not fit");
 // tip_nn_filter keeps the query tile resident for packed rows of at most this many K16 steps (d <= 128)
 constexpr int kRsMaxK16 = 9;
 
 enum { MODE_NN = 0, MODE_LSE = 1, MODE_DUMP = 2, MODE_DSUM = 3 };
+
+// Per-instantiation shape of pair_kernel.  Shared memory: [kFront: streaming ring, or resident query tile + train
+// ring] [barriers + hand-out slots] [candidate staging] [two event mailboxes].
+template <int MODE, bool RESA>
+struct Layout {
+  static constexpr int kWgs = MODE == MODE_NN && RESA ? 3 : 2;   // consumer warpgroups
+  static constexpr int kRows = 64 * kWgs;                         // query rows per tile
+  static constexpr int kConsumerWarps = 4 * kWgs;
+  static constexpr int kThreads = 128 + 32 * kConsumerWarps;
+  static constexpr int kABytes = kRows * BK * 2;                  // one resident K chunk of the query tile
+  static constexpr int kResAChunks = kWgs == 3 ? (kRsMaxK16 + 3) / 4 : tip::kResAChunks;
+  static constexpr int kFront = kWgs == 3 ? kResAChunks * kABytes + kStages * kBBytes : kRingBytes;
+  static constexpr int kCandBytes = kCandSlots * kRows * 12;      // value, chunk start, 32-bit column mask
+  static constexpr int kSmemBytes = kFront + 1024 /*align slack*/ + kBarBytes + kCandBytes + 2 * (int)sizeof(EvBuf<kRows>);
+  static_assert(!RESA || kResAChunks * kABytes + kStages * kBBytes <= kFront, "resident-query layout does not fit");
+  static_assert(kSmemBytes <= kSmemMax, "pair kernel does not fit");
+};
 
 struct PairArgs {
   const tip_work_item* items;
@@ -131,11 +145,15 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded spin: a protocol bug must surface as a trapped kernel, never as a hung GPU.
+// Bounded spin: a protocol bug must surface as a trapped kernel, never as a hung GPU.  BOUNDED = false: the consumers
+// of the resident MODE_NN kernel, because ptxas ignores setmaxnreg's larger register budget in a region that can trap
+// (and an exit there, with wgmma in flight, serialises the wgmma).  A consumer warp stuck in such a wait never hands
+// the drain warps its last mailbox, so their bounded wait traps instead.
+template <bool BOUNDED = true>
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, uint32_t max_spins = 200000000u) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if (++spins > max_spins) __trap();
+    if (BOUNDED && ++spins > max_spins) __trap();
   }
 }
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
@@ -213,7 +231,7 @@ struct EpiState {
   float run_max, run_sum;              // MODE_LSE
   double dsum;                         // MODE_DSUM
 };
-// MODE_NN per-row candidate staging: slot k of local row r at [k * BM + r]
+// MODE_NN per-row candidate staging: slot k of local row r at [k * ROWS + r] (ROWS: the tile's query rows)
 struct EpiShared {
   float* cand_val;
   int* cand_col;
@@ -222,25 +240,26 @@ struct EpiShared {
 
 // Stage chunk `col` (minimum mn, column mask) of a row with n staged chunks.  Full slots are first compacted against
 // thr (the row's current threshold); if they all stay live, the chunk goes straight to the row's list.
+template <int ROWS>
 __device__ __forceinline__ void stage_chunk(const PairArgs& args, const EpiShared& sh, int r, int& n, int64_t row,
                                             int col, uint32_t mask, float mn, float thr) {
   if (n == kCandSlots) {
     int keep = 0;
     for (int k = 0; k < kCandSlots; k++) {
-      const float sv = sh.cand_val[k * BM + r];
+      const float sv = sh.cand_val[k * ROWS + r];
       if (sv <= thr) {
-        sh.cand_val[keep * BM + r] = sv;
-        sh.cand_col[keep * BM + r] = sh.cand_col[k * BM + r];
-        sh.cand_mask[keep * BM + r] = sh.cand_mask[k * BM + r];
+        sh.cand_val[keep * ROWS + r] = sv;
+        sh.cand_col[keep * ROWS + r] = sh.cand_col[k * ROWS + r];
+        sh.cand_mask[keep * ROWS + r] = sh.cand_mask[k * ROWS + r];
         keep++;
       }
     }
     n = keep;
   }
   if (n < kCandSlots) {
-    sh.cand_val[n * BM + r] = mn;
-    sh.cand_col[n * BM + r] = col;
-    sh.cand_mask[n * BM + r] = mask;
+    sh.cand_val[n * ROWS + r] = mn;
+    sh.cand_col[n * ROWS + r] = col;
+    sh.cand_mask[n * ROWS + r] = mask;
     n++;
   } else {
     const int pos = atomicAdd(args.cand_cnt + row, 1);
@@ -251,14 +270,15 @@ __device__ __forceinline__ void stage_chunk(const PairArgs& args, const EpiShare
   }
 }
 // End of an item: emit the staged chunks of a row that survive its final threshold.
+template <int ROWS>
 __device__ __forceinline__ void flush_row(const PairArgs& args, const EpiShared& sh, int r, int n, int64_t row,
                                           float thr) {
   for (int q = 0; q < n; q++) {
-    if (sh.cand_val[q * BM + r] <= thr) {
+    if (sh.cand_val[q * ROWS + r] <= thr) {
       const int pos = atomicAdd(args.cand_cnt + row, 1);
       if (pos < args.cap) {
-        args.cand_idx[(row * args.cap + pos) * 2] = sh.cand_col[q * BM + r];
-        args.cand_idx[(row * args.cap + pos) * 2 + 1] = (int)sh.cand_mask[q * BM + r];
+        args.cand_idx[(row * args.cap + pos) * 2] = sh.cand_col[q * ROWS + r];
+        args.cand_idx[(row * args.cap + pos) * 2 + 1] = (int)sh.cand_mask[q * ROWS + r];
       }
     }
   }
@@ -315,7 +335,7 @@ __device__ __forceinline__ void epi_chunk(const PairArgs& args, EpiState& st, co
         for (int k = 0; k < 8; k++) mask |= (v[k] <= st.thr) ? (1u << (8 * (k >> 1) + 2 * sub + (k & 1))) : 0u;
         mask |= __shfl_xor_sync(qmask, mask, 1);
         mask |= __shfl_xor_sync(qmask, mask, 2);
-        if (sub == 0) stage_chunk(args, sh, etid, st.n_staged, st.row, cbase, mask, mn, st.thr);
+        if (sub == 0) stage_chunk<BM>(args, sh, etid, st.n_staged, st.row, cbase, mask, mn, st.thr);
       }
       return;
     }
@@ -390,16 +410,21 @@ __device__ __forceinline__ void epi_chunk(const PairArgs& args, EpiState& st, co
 }
 
 template <int MODE, bool EXCL, bool RESA, bool F16>
-__global__ void __launch_bounds__(kThreads, 1)
+__global__ void __launch_bounds__(Layout<MODE, RESA>::kThreads, 1)
 pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const PairArgs args) {
+  using L = Layout<MODE, RESA>;
+  constexpr int kConsumerWarps = L::kConsumerWarps;
+  // 512 threads leave 128 registers each; warpgroup 0 (producer lane, drain warps) runs on 56 and hands the rest to
+  // the consumers: 128 x 56 + 384 x 152 = 64 K
+  constexpr bool kSplitRegs = L::kWgs == 3;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
   uint8_t* smem = smem_raw + (base - raw);
   // streaming: stage s = A tile | B tile at base + s * kStageBytes.  RESA: the query tile's chunks at base, the train
   // ring behind them.
-  const uint32_t b_ring = base + (RESA ? kResAChunks * kABytes : 0);
-  const uint32_t bar0 = base + kRingBytes;
+  const uint32_t b_ring = base + (RESA ? L::kResAChunks * L::kABytes : 0);
+  const uint32_t bar0 = base + L::kFront;
   auto full_bar = [&](int s) { return bar0 + 8u * s; };
   auto empty_bar = [&](int s) { return bar0 + 8u * (kStages + s); };
   const uint32_t a_full = bar0 + 8u * (2 * kStages), a_empty = bar0 + 8u * (2 * kStages + 1);
@@ -407,13 +432,13 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   auto sched_empty = [&](int s) { return bar0 + 8u * (2 * kStages + 4 + s); };
   auto ev_full = [&](int b) { return bar0 + 8u * (2 * kStages + 6 + b); };
   auto ev_empty = [&](int b) { return bar0 + 8u * (2 * kStages + 8 + b); };
-  volatile int* sched_ring = reinterpret_cast<volatile int*>(smem + kRingBytes + 8 * (2 * kStages + 10));
+  volatile int* sched_ring = reinterpret_cast<volatile int*>(smem + L::kFront + 8 * (2 * kStages + 10));
   static_assert(8 * (2 * kStages + 10) + 8 <= kBarBytes, "barrier block");
   EpiShared sh;   // MODE_NN candidate staging: drain warps (resident variant) / consumers (streaming variant)
-  sh.cand_val = reinterpret_cast<float*>(smem + kRingBytes + kBarBytes);
-  sh.cand_col = reinterpret_cast<int*>(sh.cand_val + kCandSlots * BM);
-  sh.cand_mask = reinterpret_cast<uint32_t*>(sh.cand_col + kCandSlots * BM);
-  EvBuf* evbuf = reinterpret_cast<EvBuf*>(smem + kRingBytes + kBarBytes + kCandBytes);
+  sh.cand_val = reinterpret_cast<float*>(smem + L::kFront + kBarBytes);
+  sh.cand_col = reinterpret_cast<int*>(sh.cand_val + kCandSlots * L::kRows);
+  sh.cand_mask = reinterpret_cast<uint32_t*>(sh.cand_col + kCandSlots * L::kRows);
+  EvBuf<L::kRows>* evbuf = reinterpret_cast<EvBuf<L::kRows>*>(smem + L::kFront + kBarBytes + L::kCandBytes);
 
   // warp index through a shuffle: provably warp-uniform, so the compiler keeps the consumers' wgmma asynchronous
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
@@ -441,109 +466,114 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   const int k16 = args.k16;
   const int nchunks = (k16 + 3) >> 2;
 
-  if (warp == 0) {
-    // ================= TMA producer + item hand-out =================
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0, a_phase = 0;
-      int a_row0 = -1;    // query tile in shared memory (RESA): consecutive items of the same tile reuse it
-      long long n_tiles_done = 0, n_items_done = 0;
-      int w_static = blockIdx.x;
-      for (int k = 0;; k++) {
-        int w;
-        if (w_static < args.n_static) { w = w_static; w_static += gridDim.x; }
-        else if (args.sched_counter) {
-          w = args.n_static + atomicAdd(args.sched_counter, 1);
-          if (w >= args.n_items) w = -1;
-        } else w = -1;
-        const int slot = k & 1;
-        mbar_wait(sched_empty(slot), ((uint32_t)(k >> 1) & 1u) ^ 1u);
-        sched_ring[slot] = w;
-        mbar_arrive(sched_full(slot));
-        if (w < 0) break;
-        const tip_work_item it = args.items[w];
-        const int ntiles = (it.col1 - it.col0 + BN - 1) / BN;
-        if (ntiles <= 0) continue;   // padding entry of a balanced work list
-        n_tiles_done += ntiles; n_items_done++;
-        if (RESA && it.q_row0 != a_row0) {
-          // the consumers arrive once they start an item of another query tile, when every MMA on this one has
-          // retired (first load: passes at once)
-          mbar_wait(a_empty, a_phase ^ 1u);
-          mbar_expect_tx(a_full, (uint32_t)nchunks * kABytes);
-          for (int c = 0; c < nchunks; c++) tma_load_2d(base + (uint32_t)c * kABytes, &tmA, a_full, c * BK, it.q_row0);
-          a_phase ^= 1u;
-          a_row0 = it.q_row0;
-        }
-        for (int t = 0; t < ntiles; t++) {
-          TL(8);
-          for (int c = 0; c < nchunks; c++) {
-            mbar_wait(empty_bar(stage), phase ^ 1u);
-            if (RESA) {
-              mbar_expect_tx(full_bar(stage), kBBytes);
-              tma_load_2d(b_ring + (uint32_t)stage * kBBytes, &tmB, full_bar(stage), c * BK, it.col0 + t * BN);
-            } else {
-              mbar_expect_tx(full_bar(stage), kStageBytes);
-              const uint32_t a_dst = base + stage * kStageBytes;
-              tma_load_2d(a_dst, &tmA, full_bar(stage), c * BK, it.q_row0);
-              tma_load_2d(a_dst + kABytes, &tmB, full_bar(stage), c * BK, it.col0 + t * BN);
+  if (warp < 4) {
+    if (kSplitRegs) asm volatile("setmaxnreg.dec.sync.aligned.u32 56;" ::: "memory");
+    if (warp == 0) {
+      // ================= TMA producer + item hand-out =================
+      if (lane == 0) {
+        int stage = 0;
+        uint32_t phase = 0, a_phase = 0;
+        int a_row0 = -1;    // query tile in shared memory (RESA): consecutive items of the same tile reuse it
+        long long n_tiles_done = 0, n_items_done = 0;
+        int w_static = blockIdx.x;
+        for (int k = 0;; k++) {
+          int w;
+          if (w_static < args.n_static) { w = w_static; w_static += gridDim.x; }
+          else if (args.sched_counter) {
+            w = args.n_static + atomicAdd(args.sched_counter, 1);
+            if (w >= args.n_items) w = -1;
+          } else w = -1;
+          const int slot = k & 1;
+          mbar_wait(sched_empty(slot), ((uint32_t)(k >> 1) & 1u) ^ 1u);
+          sched_ring[slot] = w;
+          mbar_arrive(sched_full(slot));
+          if (w < 0) break;
+          const tip_work_item it = args.items[w];
+          const int ntiles = (it.col1 - it.col0 + BN - 1) / BN;
+          if (ntiles <= 0) continue;   // padding entry of a balanced work list
+          n_tiles_done += ntiles; n_items_done++;
+          if (RESA && it.q_row0 != a_row0) {
+            // the consumers arrive once they start an item of another query tile, when every MMA on this one has
+            // retired (first load: passes at once)
+            mbar_wait(a_empty, a_phase ^ 1u);
+            mbar_expect_tx(a_full, (uint32_t)nchunks * L::kABytes);
+            for (int c = 0; c < nchunks; c++)
+              tma_load_2d(base + (uint32_t)c * L::kABytes, &tmA, a_full, c * BK, it.q_row0);
+            a_phase ^= 1u;
+            a_row0 = it.q_row0;
+          }
+          for (int t = 0; t < ntiles; t++) {
+            TL(8);
+            for (int c = 0; c < nchunks; c++) {
+              mbar_wait(empty_bar(stage), phase ^ 1u);
+              if (RESA) {
+                mbar_expect_tx(full_bar(stage), kBBytes);
+                tma_load_2d(b_ring + (uint32_t)stage * kBBytes, &tmB, full_bar(stage), c * BK, it.col0 + t * BN);
+              } else {
+                mbar_expect_tx(full_bar(stage), kStageBytes);
+                const uint32_t a_dst = base + stage * kStageBytes;
+                tma_load_2d(a_dst, &tmA, full_bar(stage), c * BK, it.q_row0);
+                tma_load_2d(a_dst + kABytes, &tmB, full_bar(stage), c * BK, it.col0 + t * BN);
+              }
+              if (++stage == kStages) { stage = 0; phase ^= 1u; }
             }
-            if (++stage == kStages) { stage = 0; phase ^= 1u; }
+            TL(10);
+            tl_tile++;
           }
-          TL(10);
-          tl_tile++;
+        }
+        if (args.cta_clock) {
+          args.cta_clock[blockIdx.x * 4 + 2] = n_tiles_done;
+          unsigned smid;
+          asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
+          args.cta_clock[blockIdx.x * 4 + 3] = n_items_done | ((long long)smid << 32);
         }
       }
-      if (args.cta_clock) {
-        args.cta_clock[blockIdx.x * 4 + 2] = n_tiles_done;
-        unsigned smid;
-        asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-        args.cta_clock[blockIdx.x * 4 + 3] = n_items_done | ((long long)smid << 32);
-      }
-    }
-    __syncwarp();
-  } else if (warp < 4) {
-    // ================= MODE_NN drain (resident variant): stage the consumers' events =================
-    // Thread dt owns local rows dt and dt + 96: their staging slots and counts.  Per row, events arrive in column
-    // order.  An event is staged unless it is dead against the tighter of the record's thr and the row's thr after
-    // its tile; with the slots full they are compacted against that threshold, and a chunk that still finds them
-    // full of live chunks goes straight to the row's list.  The last tile of an item flushes the slots that
-    // survive the row's final thr (read by the consumers after the item, from the shared running minimum).
-    if (MODE == MODE_NN && RESA) {
-      const int dt = threadIdx.x - 32;
-      int n_staged[2] = {0, 0};
-      for (int qt = 0;; qt++) {
-        const int b = qt & 1;
-        mbar_wait(ev_full(b), (uint32_t)(qt >> 1) & 1u);
-        const EvBuf& e = evbuf[b];
-        const int flags = e.flags;
-        if (flags & kEvStop) break;
-        const bool stamp = args.timeline && blockIdx.x == 0 && dt == 0 && qt < args.timeline_tiles;
-        if (stamp) args.timeline[(int64_t)qt * 16 + 11] = clock64();
+      __syncwarp();
+    } else {
+      // ================= MODE_NN drain (resident variant): stage the consumers' events =================
+      // Thread dt owns local rows dt and dt + 96 of the 192-row tile: their staging slots and counts.  Per row, events arrive in column
+      // order.  An event is staged unless it is dead against the tighter of the record's thr and the row's thr after
+      // its tile; with the slots full they are compacted against that threshold, and a chunk that still finds them
+      // full of live chunks goes straight to the row's list.  The last tile of an item flushes the slots that
+      // survive the row's final thr (read by the consumers after the item, from the shared running minimum).
+      if (MODE == MODE_NN && RESA) {
+        static_assert(!(MODE == MODE_NN && RESA) || L::kRows == 2 * 32 * kDrainWarps, "two rows per drain thread");
+        const int dt = threadIdx.x - 32;
+        int n_staged[2] = {0, 0};
+        for (int qt = 0;; qt++) {
+          const int b = qt & 1;
+          mbar_wait(ev_full(b), (uint32_t)(qt >> 1) & 1u);
+          const EvBuf<L::kRows>& e = evbuf[b];
+          const int flags = e.flags;
+          if (flags & kEvStop) break;
+          const bool stamp = args.timeline && blockIdx.x == 0 && dt == 0 && qt < args.timeline_tiles;
+          if (stamp) args.timeline[(int64_t)qt * 16 + 11] = clock64();
 #pragma unroll
-        for (int j = 0; j < 2; j++) {
-          const int r = dt + 32 * kDrainWarps * j;
-          if (r >= BM) continue;
-          const EvRow er = e.row[r];
-          const int64_t row = (int64_t)e.q_row0 + r;
-          for (int c = 0; c < kEvSlots; c++) {
-            if (!((er.ev >> c) & 1)) continue;
-            const EvRecord rc = e.rec[r * kEvSlots + c];
-            const float thr = fminf(rc.thr, er.thr);
-            if (rc.mn <= thr) stage_chunk(args, sh, r, n_staged[j], row, rc.col, rc.mask, rc.mn, thr);
+          for (int j = 0; j < 2; j++) {
+            const int r = dt + 32 * kDrainWarps * j;
+            const EvRow er = e.row[r];
+            const int64_t row = (int64_t)e.q_row0 + r;
+            for (int c = 0; c < kEvSlots; c++) {
+              if (!((er.ev >> c) & 1)) continue;
+              const EvRecord rc = e.rec[r * kEvSlots + c];
+              const float thr = fminf(rc.thr, er.thr);
+              if (rc.mn <= thr) stage_chunk<L::kRows>(args, sh, r, n_staged[j], row, rc.col, rc.mask, rc.mn, thr);
+            }
+            if (flags & kEvLast) {
+              flush_row<L::kRows>(args, sh, r, n_staged[j], row, er.thr);
+              n_staged[j] = 0;
+            }
           }
-          if (flags & kEvLast) {
-            flush_row(args, sh, r, n_staged[j], row, er.thr);
-            n_staged[j] = 0;
-          }
+          if (stamp) args.timeline[(int64_t)qt * 16 + 12] = clock64();
+          __syncwarp();
+          if (lane == 0) mbar_arrive(ev_empty(b));
         }
-        if (stamp) args.timeline[(int64_t)qt * 16 + 12] = clock64();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(ev_empty(b));
       }
     }
   } else {
     // ================= consumers: wgmma + register epilogue =================
-    const int cw = warp - 4;                    // consumer warp 0..7
+    if (kSplitRegs) asm volatile("setmaxnreg.inc.sync.aligned.u32 152;" ::: "memory");
+    const int cw = warp - 4;                    // consumer warp 0 .. kConsumerWarps - 1
     const int g = cw >> 2;                        // consumer warpgroup: query rows [64 g, 64 g + 64)
     const int sub = lane & 3;
     const int lead = lane & 28;                   // the quad's first lane
@@ -559,13 +589,13 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     int qt = 0;                 // MODE_NN: tiles handed to the drain so far (mailbox qt & 1)
     for (int k = 0;; k++) {
       const int slot = k & 1;
-      mbar_wait(sched_full(slot), (uint32_t)(k >> 1) & 1u);
+      mbar_wait<!kSplitRegs>(sched_full(slot), (uint32_t)(k >> 1) & 1u);
       const int w = sched_ring[slot];
       __syncwarp();
       if (lane == 0) mbar_arrive(sched_empty(slot));
       if (w < 0) {
         if (MODE == MODE_NN && RESA) {   // release the drain warps
-          mbar_wait(ev_empty(qt & 1), ((uint32_t)(qt >> 1) & 1u) ^ 1u);
+          mbar_wait<!kSplitRegs>(ev_empty(qt & 1), ((uint32_t)(qt >> 1) & 1u) ^ 1u);
           if (cw == 0 && lane == 0) evbuf[qt & 1].flags = kEvStop;
           __syncwarp();
           if (lane == 0) mbar_arrive(ev_full(qt & 1));
@@ -575,6 +605,9 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       const tip_work_item it = args.items[w];
       const int ntiles = (it.col1 - it.col0 + BN - 1) / BN;
       if (ntiles <= 0) continue;
+      // a warpgroup whose 64 rows all lie past the item's query rows issues no MMAs; with no valid row its epilogue
+      // only hands empty mailbox entries to the drain, and it keeps its place in the ring and query-tile protocols
+      const bool idle = L::kWgs == 3 && __shfl_sync(0xffffffffu, (int)(64 * g >= it.q_rows), 0);
       EpiState st[2];
 #pragma unroll
       for (int h = 0; h < 2; h++) {
@@ -616,7 +649,7 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
           __syncwarp();
           if (lane == 0) mbar_arrive(a_empty);
         }
-        mbar_wait(a_full, a_phase);
+        mbar_wait<!kSplitRegs>(a_full, a_phase);
         a_phase ^= 1u;
         a_row0 = it.q_row0;
       }
@@ -633,9 +666,16 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       auto issue_tile = [&](float (&a)[64], int t) {
         TLT(t, 0);
         acc_fence(a);
+        if (idle) {   // the tile's stages are released with everybody else's
+          for (int c = 0; c < nchunks; c++) {
+            mbar_wait<!kSplitRegs>(full_bar(stage), phase);
+            if (++stage == kStages) { stage = 0; phase ^= 1u; }
+          }
+          return;
+        }
         for (int c = 0; c < nchunks; c++) {
-          mbar_wait(full_bar(stage), phase);
-          const uint32_t a_addr = base + (uint32_t)c * kABytes + (uint32_t)g * 64 * 128;
+          mbar_wait<!kSplitRegs>(full_bar(stage), phase);
+          const uint32_t a_addr = base + (uint32_t)c * L::kABytes + (uint32_t)g * 64 * 128;
           const uint32_t b_addr = b_ring + (uint32_t)stage * kBBytes;
           const uint64_t adesc = smem_desc(a_addr), bdesc = smem_desc(b_addr);
           const int nm = min(4, k16 - 4 * c);
@@ -669,10 +709,10 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         const int col_base = it.col0 + t * BN;
         const bool partial = col_base + BN > it.col1;
         const bool last = t == ntiles - 1;
-        EvBuf* eb = evbuf + (qt & 1);
+        EvBuf<L::kRows>* eb = evbuf + (qt & 1);
         int ev[2] = {0, 0};
         // a free mailbox (convergent: the drain released it two tiles ago)
-        if (MODE == MODE_NN) mbar_wait(ev_empty(qt & 1), ((uint32_t)(qt >> 1) & 1u) ^ 1u);
+        if (MODE == MODE_NN) mbar_wait<!kSplitRegs>(ev_empty(qt & 1), ((uint32_t)(qt >> 1) & 1u) ^ 1u);
         if (MODE == MODE_DUMP) {
           if (dump_item && t < 2) {     // the first 128 rows x 256 columns of the first item
 #pragma unroll
@@ -761,7 +801,7 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         for (int t = 0; t < ntiles; t++) {
           TLT(t, 0);
           for (int c = 0; c < nchunks; c++) {
-            mbar_wait(full_bar(stage), phase);
+            mbar_wait<!kSplitRegs>(full_bar(stage), phase);
             const uint32_t a_addr = base + stage * kStageBytes + (uint32_t)g * 64 * 128;
             const uint32_t b_addr = base + stage * kStageBytes + kABytes;
             const uint64_t adesc = smem_desc(a_addr), bdesc = smem_desc(b_addr);
@@ -843,7 +883,7 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             s.s_ref = seen;
             s.thr = nn_threshold(s.s_ref, s.nx, s.e2, s.g);
           }
-          flush_row(args, sh, row_h0 + 8 * h, s.n_staged, s.row, s.thr);
+          flush_row<BM>(args, sh, row_h0 + 8 * h, s.n_staged, s.row, s.thr);
         } else if (MODE == MODE_LSE) {
           args.part_max[(int64_t)it.slot * args.m + s.row] = s.run_max;
           args.part_sum[(int64_t)it.slot * args.m + s.row] = s.run_sum;
@@ -909,32 +949,34 @@ static int check_device() {
   return TIP_OK;
 }
 
-// resa: the query tile stays resident in shared memory for each work item (needs <= kResAChunks K chunks)
+// resa: the query tile stays resident in shared memory for each work item (needs <= Layout::kResAChunks K chunks)
 template <int MODE, bool EXCL = false, bool F16 = false>
 static int launch_pair(const void* q_pack, int64_t m, const void* t_pack, int64_t n, int64_t pitch, PairArgs args,
                        bool resa, cudaStream_t st) {
+  using LS = Layout<MODE, false>;
+  using LR = Layout<MODE, true>;
   int rc = check_device();
   if (rc != TIP_OK) return rc;
   TIP_REQUIRE(((uintptr_t)q_pack & 127) == 0 && ((uintptr_t)t_pack & 127) == 0, "packed operands must be 128-byte aligned");
   TIP_REQUIRE(pitch % 64 == 0 && args.k16 >= 1 && args.k16 * 16 <= pitch, "pitch");
   TIP_REQUIRE(m >= 1 && n >= 1 && m < (1LL << 31) && n < (1LL << 31), "shape");
-  TIP_REQUIRE(!resa || (args.k16 + 3) / 4 <= kResAChunks, "packed width too large for the resident-query kernel");
+  TIP_REQUIRE(!resa || (args.k16 + 3) / 4 <= LR::kResAChunks, "packed width too large for the resident-query kernel");
   CUtensorMap ma, mb;
-  rc = make_map(&ma, q_pack, m, pitch, BM);
+  rc = make_map(&ma, q_pack, m, pitch, resa ? LR::kRows : LS::kRows);
   if (rc != TIP_OK) return rc;
   rc = make_map(&mb, t_pack, n, pitch, BN);
   if (rc != TIP_OK) return rc;
   static bool attr_set = false;   // one flag per template instantiation
   if (!attr_set) {
-    TIP_CHECK_CUDA(cudaFuncSetAttribute(pair_kernel<MODE, EXCL, false, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
-    TIP_CHECK_CUDA(cudaFuncSetAttribute(pair_kernel<MODE, EXCL, true, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
+    TIP_CHECK_CUDA(cudaFuncSetAttribute(pair_kernel<MODE, EXCL, false, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, LS::kSmemBytes));
+    TIP_CHECK_CUDA(cudaFuncSetAttribute(pair_kernel<MODE, EXCL, true, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, LR::kSmemBytes));
     attr_set = true;
   }
   const int grid = std::min(args.n_items, sm_count());
   if (resa)
-    pair_kernel<MODE, EXCL, true, F16><<<grid, kThreads, kSmemBytes, st>>>(ma, mb, args);
+    pair_kernel<MODE, EXCL, true, F16><<<grid, LR::kThreads, LR::kSmemBytes, st>>>(ma, mb, args);
   else
-    pair_kernel<MODE, EXCL, false, F16><<<grid, kThreads, kSmemBytes, st>>>(ma, mb, args);
+    pair_kernel<MODE, EXCL, false, F16><<<grid, LS::kThreads, LS::kSmemBytes, st>>>(ma, mb, args);
   TIP_LAUNCH_CHECK();
   return TIP_OK;
 }
@@ -996,7 +1038,7 @@ extern "C" int tip_nn_filter(const void* q_pack, const float* q_sqnorm, int64_t 
 
 extern "C" int tip_nn_filter_tile(int64_t d, int32_t* q_rows, int32_t* t_rows) {
   TIP_REQUIRE(d >= 1 && q_rows && t_rows, "arguments");
-  *q_rows = BM;
+  *q_rows = tip_nn_filter_kind(d) == 1 ? Layout<MODE_NN, true>::kRows : Layout<MODE_NN, false>::kRows;
   *t_rows = BN;
   return TIP_OK;
 }
