@@ -195,8 +195,12 @@ int tip_cover_threshold(const void* act, int act_dtype, int64_t n, int64_t d, co
 /* Top-k neuron coverage of ONE layer (neuron_coverage.py:160-168): for every sample the k largest of its
  * d_layer activations are marked in profile_u8[r * row_stride + col_off + i] (all entries of the layer's
  * columns are written) and/or OR-ed into the packed words of neuron col_off + i (bits must be zero-filled
- * by the caller; bit_words = words per row).  Equal values: the higher index wins (NumPy's unstable
- * argsort leaves that case implementation-defined). */
+ * by the caller; bit_words = words per row).  k >= 0 is the number of neurons marked: the caller passes
+ * len(range(d_layer)[-top_neurons:]), the count the reference's slice `argsort(layer)[..., -top_neurons:]`
+ * takes (d_layer for top_neurons = 0, d_layer - |top_neurons| for negative values); k >= d_layer marks the
+ * whole layer without running the k block-wide selection rounds.  Equal values: the higher index wins, NaN
+ * ranks above everything (a stable ascending argsort's last entries; NumPy's unstable argsort leaves ties
+ * implementation-defined). */
 int tip_tknc(const void* act, int dtype, int64_t n, int64_t d_layer, int32_t k, void* profile_u8,
              int64_t row_stride, int64_t col_off, uint32_t* bits, int64_t bit_words, void* stream);
 /* Streaming per-neuron statistics over a batch of n samples x d neurons: mins/maxs and welford==0.2.5's

@@ -281,6 +281,40 @@ def sibling_cases(ref):
     print("siblings ok", {k: int(out[f"sib.{k}.score"].sum()) for k in metrics})
 
 
+def coverage_edge_cases(ref):
+    """The reference's TKNC at k <= 0 and k >= d (its slice `argsort(layer)[..., -k:]` marks every neuron for k = 0
+    and all but the |k| lowest for k < 0) on tie-free layers, and its NAC on activations that are not float32 /
+    float64 (`activations > threshold` compares in NumPy's promotion of the activation dtype with a Python float)."""
+    nc = ref.neuron_coverage
+    out = {}
+    rng = np.random.default_rng(97)
+    widths = (1, 5, 37)
+    # a permutation per row: distinct values in every row, so the reference's unstable argsort has no ties to break
+    layers = [(np.stack([rng.permutation(w) for _ in range(9)]) * 0.37 - 2).astype(np.float32) for w in widths]
+    for i, l in enumerate(layers):
+        out[f"tknc.layer{i}"] = l
+    d = sum(widths)
+    for k in (0, -1, -3, d, d + 2):
+        score, prof = nc.TKNC(k)([l.copy() for l in layers])
+        out[f"tknc.k{k}.score"], out[f"tknc.k{k}.profile"] = score, prof
+    grid = np.array([0.3, 0.75, 1.9999999999, 2.0, 1.0, 0.0, -1.0]).astype(np.float16)   # and one float16 ulp either side
+    acts = {
+        "f16": np.concatenate([grid, np.nextafter(grid, np.float16(3)), np.nextafter(grid, np.float16(-3)),
+                               rng.normal(size=11).astype(np.float16)]),
+        "i16": np.array([-3, -1, 0, 1, 2, 3, 300, -300], dtype=np.int16),
+        "u8": np.array([0, 1, 2, 3, 255], dtype=np.uint8),
+        "bool": np.array([False, True]),
+    }
+    for name, a in acts.items():
+        a = np.resize(a, 2 * a.size).reshape(2, -1)
+        out[f"nac.{name}.act"] = a
+        for t in (0.3, 0.75, 0.9999999999, 1.9999999999):
+            score, prof = nc.NAC(t)([a.copy()])
+            out[f"nac.{name}.{t!r}.score"], out[f"nac.{name}.{t!r}.profile"] = score, prof
+    np.savez_compressed(os.path.join(OUT, "coverage_edges_reference.npz"), **out)
+    print("coverage edges ok", {k: int(out[f"tknc.k{k}.score"][0]) for k in (0, -1, -3, d, d + 2)})
+
+
 def mdsa_mlsa_cases(ref):
     """MDSA / MLSA (surprise.py:374-393,498-520) and their per-class forms (handler_surprise.py:28-33) run by the
     reference's own classes on top of this container's scikit-learn.  GaussianMixture's fit draws from NumPy's
@@ -319,6 +353,9 @@ if __name__ == "__main__":
     if len(sys.argv) > 1 and sys.argv[1] == "siblings":
         sibling_cases(ref)
         sys.exit(0)
+    if len(sys.argv) > 1 and sys.argv[1] == "coverage_edges":
+        coverage_edge_cases(ref)
+        sys.exit(0)
     dsa_cases(ref)
     lsa_cases(ref)
     coverage_cases(ref)
@@ -327,4 +364,5 @@ if __name__ == "__main__":
     cam_kmnc_cases(ref)
     sibling_cases(ref)
     mdsa_mlsa_cases(ref)
+    coverage_edge_cases(ref)
     print("sizes:", {f: os.path.getsize(os.path.join(OUT, f)) for f in sorted(os.listdir(OUT))})

@@ -49,8 +49,10 @@ class CoverageMethod(abc.ABC):
 
 def _device_activations(activations):
     """Activations (NumPy array / list of layers / torch CUDA tensors) as one contiguous [N, D] matrix in
-    HBM plus its NumPy dtype; float32 / float64 are kept, everything else is scored in float32... after
-    NumPy's promotion with the boundaries (done by the caller)."""
+    HBM, its NumPy dtype there, and the NumPy dtype the activations came in.  float32 / float64 are kept;
+    everything else is widened exactly (float16, bool and small integers to float32, wider integers to
+    float64).  The comparison dtype is NumPy's promotion of the ORIGINAL dtype with the boundaries (the
+    caller's job).  A torch bfloat16 tensor has no NumPy dtype: it counts as float32."""
     import torch
 
     from .. import engine as E
@@ -58,19 +60,25 @@ def _device_activations(activations):
     dev = E.require_cuda()
     dev_act = E.device_matrix(activations)
     if dev_act is not None:
-        act = dev_act if dev_act.dtype in (torch.float32, torch.float64) else dev_act.to(torch.float32)
-        return act.contiguous(), E.NP_DTYPE[act.dtype]
+        orig = np.dtype(np.float32) if dev_act.dtype == torch.bfloat16 else torch.empty(0, dtype=dev_act.dtype).numpy().dtype
+        wide = np.result_type(orig, np.float32)
+        if wide not in (np.float32, np.float64):
+            raise TypeError(f"unsupported activation dtype {dev_act.dtype}")
+        act = dev_act if dev_act.dtype in (torch.float32, torch.float64) else dev_act.to(
+            torch.float64 if wide == np.float64 else torch.float32)
+        return act.contiguous(), E.NP_DTYPE[act.dtype], orig
     if isinstance(activations, np.ndarray):
         act = activations.reshape((activations.shape[0], -1))
     elif len(activations) == 1:
         act = np.reshape(activations[0], (activations[0].shape[0], -1))
     else:
         act = flatten_layers(activations)
+    orig = act.dtype
     if act.dtype not in (np.float32, np.float64):
         act = act.astype(np.result_type(act.dtype, np.float32))
         if act.dtype not in (np.float32, np.float64):
             raise TypeError(f"unsupported activation dtype {act.dtype}")
-    return E.to_device(act, dev), act.dtype
+    return E.to_device(act, dev), act.dtype, orig
 
 
 class _ThresholdCoverage(CoverageMethod):
@@ -90,7 +98,7 @@ class _ThresholdCoverage(CoverageMethod):
         from .. import engine as E
 
         lib = _lib.load()
-        act, act_dt = _device_activations(activations)
+        act, act_dt, orig_dt = _device_activations(activations)
         dev = act.device
         n, d = act.shape
         lo, hi, thr = self._bounds()
@@ -107,12 +115,14 @@ class _ThresholdCoverage(CoverageMethod):
             lo_dev, hi_dev = self._dev_lo, self._dev_hi
             thr_val = 0.0
         else:
-            # NAC: `activations > threshold` with a Python / NumPy scalar: NumPy compares in the promoted dtype
-            stat_dt = np.result_type(act_dt, thr)
-            if stat_dt not in (np.float32, np.float64):
-                stat_dt = np.dtype(np.float64)
+            # NAC: `activations > threshold` with a Python / NumPy scalar: NumPy compares in the promotion of the
+            # activations' own dtype with the threshold (float16 stays float16, int16 against a Python float is
+            # float64).  The threshold is rounded to that dtype; the kernel then compares in float64 when it is
+            # float64 or an integer type, else in float32, which is exact for float16 values.
+            cmp_dt = np.result_type(orig_dt, thr)
+            stat_dt = np.dtype(np.float32) if cmp_dt in (np.float16, np.float32) else np.dtype(np.float64)
             lo_dev = hi_dev = None
-            thr_val = float(np.asarray(thr).astype(stat_dt))
+            thr_val = float(np.asarray(thr).astype(cmp_dt)) if cmp_dt.kind == "f" else float(thr)
         profile = torch.empty((n, d) if self._planes == 1 else (n, d, 2), dtype=torch.bool, device=dev) if want_profile else None
         words = int(lib.tip_cover_packed_words(d))
         bits = torch.empty((n, self._planes * words), dtype=torch.int32, device=dev) if want_bits else None
@@ -352,7 +362,8 @@ class SNAC(_ThresholdCoverage):
 class TKNC(CoverageMethod):
     """Top-k neuron coverage, per layer (neuron_coverage.py:151-173).  Equal activations at the k-th rank:
     the higher index is marked (NumPy's unstable argsort leaves that case open; the reference's own test
-    accepts either outcome)."""
+    accepts either outcome).  Each layer of d neurons marks `len(range(d)[-k:])` of them, as the reference's slice
+    does: every neuron for k = 0 or k >= d, all but the |k| lowest for k < 0."""
 
     def __init__(self, top_neurons: int):
         super().__init__()
@@ -382,12 +393,14 @@ class TKNC(CoverageMethod):
         profile = torch.empty((n, total), dtype=torch.bool, device=dev) if want_profile else None
         words = int(lib.tip_cover_packed_words(total))
         bits = torch.zeros((n, words), dtype=torch.int32, device=dev) if want_bits else None
-        off = 0
+        off = score = 0
         for l in layers:
-            _lib.check(lib.tip_tknc(E._p(l), E.tip_dtype(l.dtype), n, l.shape[1], int(self.top_neurons), E._p(profile),
+            # the reference marks `np.argsort(layer)[..., -k:]`: k = 0 marks every neuron, k < 0 all but the |k| lowest
+            count = len(range(int(l.shape[1]))[-int(self.top_neurons):])
+            _lib.check(lib.tip_tknc(E._p(l), E.tip_dtype(l.dtype), n, l.shape[1], count, E._p(profile),
                                     total, off, E._p(bits), words, E._stream()), "tip_tknc")
             off += int(l.shape[1])
-        score = sum(min(int(self.top_neurons), int(l.shape[1])) for l in layers)
+            score += count
         return score, profile, bits, n, total
 
     def __call__(self, activations):

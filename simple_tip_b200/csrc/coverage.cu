@@ -121,7 +121,7 @@ __global__ void __launch_bounds__(256) cover_threshold_kernel(const TA* __restri
 
 // ---- TKNC -------------------------------------------------------------------------------------------
 // One block per sample: k rounds of "largest remaining value" over the layer held in registers/shared
-// memory.  Ties at equal values go to the HIGHER index (where a stable ascending argsort puts them last);
+// memory; k >= d_layer marks the whole layer without any round.  Ties at equal values go to the HIGHER index (where a stable ascending argsort puts them last);
 // NumPy's own argsort is not stable, so for tied values the reference's choice is implementation-defined
 // (its test accepts either, tests/test_coverage_metrics.py:157-162).
 template <typename T>
@@ -134,9 +134,10 @@ __global__ void __launch_bounds__(256) tknc_kernel(const T* __restrict__ act, in
   __shared__ long long s_idx[8];
   const int64_t r = blockIdx.x;
   const T* x = act + r * d_layer;
-  for (int64_t i = threadIdx.x; i < d_layer; i += 256) taken[i] = 0;
+  const bool all = k >= d_layer;                  // the whole layer: no rounds
+  for (int64_t i = threadIdx.x; i < d_layer; i += 256) taken[i] = all;
   __syncthreads();
-  const int kk = k < d_layer ? k : (int)d_layer;
+  const int kk = all ? 0 : k;
   for (int round = 0; round < kk; round++) {
     double bv = -INFINITY;
     long long bi = -1;
