@@ -629,7 +629,7 @@ class DSA(SA):
         self.badge_size = badge_size          # kept for API compatibility; tiles replace badges
         self.use_filter = os.environ.get("B200TIP_DSA_EXHAUSTIVE", "0") != "1"
         self.use_graphs = os.environ.get("B200TIP_GRAPHS", "1") != "0"   # CUDA-graph replay of the search
-        self.capture_on_first_call = os.environ.get("B200TIP_CAPTURE_FIRST", "0") == "1"
+        self.capture_on_first_call = False
         self._seen_shapes = set()
         self._comm = comm
         self._engine = None

@@ -27,13 +27,11 @@ import torch
 
 from . import _lib
 
-POOL_FRAC = float(os.environ.get("B200TIP_POOL_FRAC", "0.2"))   # share of the filter's work handed out dynamically
-SPECULATIVE = os.environ.get("B200TIP_SPECULATIVE", "1") != "0"   # graph plans without exhaustive-scan launches
+POOL_FRAC = 0.2           # share of the filter's work handed out dynamically
 POOL_MIN_TILES = 32       # tiles per CTA below which work lists stay purely static
-POOL_TILES = int(os.environ.get("B200TIP_POOL_TILES", "4"))      # train tiles per dynamic item
+POOL_TILES = 4            # train tiles per dynamic item
 DEFAULT_CAP = 64          # candidate chunks per query (short traces)
 DEFAULT_CAP_LONG = 256    # long traces: distances concentrate, more rows fall inside the window
-SEEDS = os.environ.get("B200TIP_SEEDS", "1") != "0"      # fit-time upper bounds that seed stage 2's running minima
 
 # bench.py sets this to a list to collect (kernel name, algorithmic flops, start event, end event)
 # around the tensor-core launches; None (default) records nothing.
@@ -609,7 +607,7 @@ class NnEngine:
         # distance to the nearest one inside a fixed stratified sample of the training set, found once at fit time
         # with this very engine machinery.
         self.seed_b = None
-        if seeds and SEEDS and self.n >= 4096 and self.num_classes >= 2 and self.resident:
+        if seeds and self.n >= 4096 and self.num_classes >= 2 and self.resident:
             self.seed_b = self._other_class_seeds()
         # Optional fit-time table (build_other_class_table): dist_b of surprise.py:622-631 depends on the test input
         # only through WHICH train row won stage 1, so it can be tabulated per train row once per training set.
@@ -980,7 +978,7 @@ class DsaPlan:
         # Single shard with the filter on: the replayed graph has NO exhaustive-scan launches (two normally empty
         # launches per call); queries whose candidate list is empty or overflowed are only counted, and the caller
         # repeats such a call on the eager path (overflowed() / clear_overflow()).
-        self.speculative = bool(use_filter and not sharded and SPECULATIVE)
+        self.speculative = bool(use_filter and not sharded)
         self.overflow = engine.work_buffer(self.m, dtype)[:4].view(torch.int32)
         self.overflow_host = torch.zeros(1, dtype=torch.int32).pin_memory()
         self._keep_alive = []
@@ -1173,8 +1171,7 @@ class KdeEngine:
                                               F16_NORM_SCALE, _p(self.t_pack_f16), None, _p(self.flags), _stream()),
                    "tip_pair_prep_f16")
         torch.cuda.current_stream().synchronize()
-        self.fast_ok = (os.environ.get("B200TIP_LSA_FAST", "1") != "0" and int(self.flags.item()) == 0
-                        and self.comm is None)
+        self.fast_ok = int(self.flags.item()) == 0 and self.comm is None
         if not self.fast_ok:
             self.t_pack_f16 = None
         self._items = {}

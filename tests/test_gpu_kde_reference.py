@@ -365,9 +365,8 @@ def test_kde_combine_is_exact_on_unit_partials(slots):
 
 # ---- the engine end to end on the exact construction -----------------------------------------------------------
 @pytest.mark.parametrize("m, n, d", [(129, 1000, 17), (500, 70_001, 97), (1030, 3000, 304)])
-def test_engine_log_kernel_sum_exact(m, n, d, monkeypatch):
+def test_engine_log_kernel_sum_exact(m, n, d):
     torch, _, _, E = _env()
-    monkeypatch.delenv("B200TIP_LSA_FAST", raising=False)
     q, p = KO.int_lse_operands(m, n, d, seed=n + d)
     eng = E.KdeEngine(p)
     assert eng.fast_ok and eng.t_pack_f16 is not None
@@ -387,11 +386,10 @@ def test_engine_log_kernel_sum_exact(m, n, d, monkeypatch):
               f"{float(np.max(np.abs(sm - want_sm))):.3g}")
 
 
-def test_fit_time_f16_range_check(monkeypatch):
+def test_fit_time_f16_range_check():
     """a training row whose norm term -|p|^2 / 2 / 64 just leaves fp16's range retires the fast operand at fit time;
     just inside it does not (|p|^2 = 2896^2 = 8 386 816 > 64 * 2 * 65504 >= 2895^2)"""
     _, _, _, E = _env()
-    monkeypatch.delenv("B200TIP_LSA_FAST", raising=False)
     rng = np.random.default_rng(9)
     p = rng.normal(size=(300, 4)) * 0.5
     for value, ok in ((2896.0, False), (2895.0, True)):
