@@ -27,10 +27,10 @@
 // Resident-query variant (RESA, short packed rows): the query tile's K chunks are loaded once per run
 // of consecutive work items on the same query tile, the ring carries train chunks only, and a tile's
 // MMAs form one commit group whose stages are released after its wait.
-// MODE_NN events, resident variant: a consumer quad that finds a chunk inside its row's window only
-// updates its running minimum and writes one record into the tile's mailbox (two, by tile parity, with
-// full/empty mbarriers); the drain warps own the per-row candidate staging (compaction, direct emission
-// when full, the flush at the end of an item).  With no data-dependent staging or divergent shuffles in
+// MODE_NN events, resident variant: per row and tile the consumers reduce all four 32-column chunks in one pass,
+// move the running minimum and threshold once, to the tile's minimum, and write one record per chunk inside that
+// end-of-tile threshold into the tile's mailbox (two, by tile parity, with full/empty mbarriers); the drain warps
+// own the per-row candidate staging (compaction, direct emission when full, the flush at the end of an item).  With no data-dependent staging or divergent shuffles in
 // the consumers' tile loop, ptxas keeps the wgmma asynchronous: a tile's HGMMAs issue back to back.
 // Streaming variant: the quad's first lane stages its events itself; there ptxas still serialises the
 // wgmma (C7520), which costs little next to the per-chunk waits, and moving the staging to the drain
@@ -299,14 +299,12 @@ __device__ __forceinline__ uint32_t ld_volatile_u32(const uint32_t* p) {
 // Reduce the 32 accumulator columns [cbase, cbase + 32) of one query row.  The row's quad holds them:
 // lane `sub` (0..3) has v[2 jj + e] = column cbase + 8 jj + 2 sub + e.  Every lane of the warp calls
 // this (the quad shuffles need the whole warp); the running state comes out the same in the four lanes
-// of a quad.  MODE_NN, resident variant: an event (a value inside the row's window) only sets bit c of `ev` and,
-// from the quad's first lane, writes the row's record for chunk c of the tile (rec); the drain warps stage and emit
-// it.  Keeping data-dependent staging out of this loop is what lets ptxas leave the wgmma asynchronous (no C7520).
-// Streaming variant (its MMAs are waited for chunk by chunk anyway): the quad's first lane stages the event itself
-// (etid = the row's staging column).
-template <int MODE, bool EXCL, bool RESA>
-__device__ __forceinline__ void epi_chunk(const PairArgs& args, EpiState& st, const EpiShared& sh, EvRecord* rec,
-                                          int& ev, float (&v)[8], int cbase, int c, int sub, bool partial, int etid) {
+// of a quad.  MODE_NN here is the streaming variant only (its MMAs are waited for chunk by chunk anyway): the quad's
+// first lane stages an event (a chunk inside the row's window) itself (etid = the row's staging column).  The resident
+// variant reduces a whole tile per row in one pass in pair_kernel's epilogue.
+template <int MODE, bool EXCL>
+__device__ __forceinline__ void epi_chunk(const PairArgs& args, EpiState& st, const EpiShared& sh, float (&v)[8],
+                                          int cbase, int sub, bool partial, int etid) {
   const float kInf = __int_as_float(0x7f800000);
   if (MODE == MODE_NN) {
     if (partial || (EXCL && cbase < st.ex_hi && cbase + 32 > st.ex_lo)) {
@@ -321,39 +319,19 @@ __device__ __forceinline__ void epi_chunk(const PairArgs& args, EpiState& st, co
     mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, 1));
     mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, 2));
     // event: this chunk holds a value inside the acceptance window of this query (quad-uniform)
-    const bool event = st.valid_row && mn <= st.thr && mn < kInf;
-    if (!RESA) {
-      if (event) {
-        if (mn < st.best) {
-          st.best = mn;
-          st.s_ref = fminf(st.s_ref, fmaxf(st.best + st.nx, 0.f));
-          st.thr = nn_threshold(st.s_ref, st.nx, st.e2, st.g);
-        }
-        const unsigned qmask = 0xFu << ((threadIdx.x & 31) & 28);   // the lanes of this quad
-        uint32_t mask = 0;
-#pragma unroll
-        for (int k = 0; k < 8; k++) mask |= (v[k] <= st.thr) ? (1u << (8 * (k >> 1) + 2 * sub + (k & 1))) : 0u;
-        mask |= __shfl_xor_sync(qmask, mask, 1);
-        mask |= __shfl_xor_sync(qmask, mask, 2);
-        if (sub == 0) stage_chunk<BM>(args, sh, etid, st.n_staged, st.row, cbase, mask, mn, st.thr);
+    if (st.valid_row && mn <= st.thr && mn < kInf) {
+      if (mn < st.best) {
+        st.best = mn;
+        st.s_ref = fminf(st.s_ref, fmaxf(st.best + st.nx, 0.f));
+        st.thr = nn_threshold(st.s_ref, st.nx, st.e2, st.g);
       }
-      return;
-    }
-    if (event && mn < st.best) {
-      st.best = mn;
-      st.s_ref = fminf(st.s_ref, fmaxf(st.best + st.nx, 0.f));
-      st.thr = nn_threshold(st.s_ref, st.nx, st.e2, st.g);
-    }
-    // exact per-column mask of the chunk: the re-rank then touches only rows inside the window.  Built by the whole
-    // warp (used only on an event): shuffles inside the divergent event branch make ptxas serialise the wgmma.
-    uint32_t mask = 0;
+      const unsigned qmask = 0xFu << ((threadIdx.x & 31) & 28);   // the lanes of this quad
+      uint32_t mask = 0;
 #pragma unroll
-    for (int k = 0; k < 8; k++) mask |= (v[k] <= st.thr) ? (1u << (8 * (k >> 1) + 2 * sub + (k & 1))) : 0u;
-    mask |= __shfl_xor_sync(0xffffffffu, mask, 1);
-    mask |= __shfl_xor_sync(0xffffffffu, mask, 2);
-    if (event) {
-      ev |= 1 << c;
-      if (sub == 0) rec[c] = EvRecord{cbase, mask, mn, st.thr};
+      for (int k = 0; k < 8; k++) mask |= (v[k] <= st.thr) ? (1u << (8 * (k >> 1) + 2 * sub + (k & 1))) : 0u;
+      mask |= __shfl_xor_sync(qmask, mask, 1);
+      mask |= __shfl_xor_sync(qmask, mask, 2);
+      if (sub == 0) stage_chunk<BM>(args, sh, etid, st.n_staged, st.row, cbase, mask, mn, st.thr);
     }
   } else if (MODE == MODE_LSE) {
     constexpr float kL2e = 1.4426950408889634f;
@@ -713,6 +691,7 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         int ev[2] = {0, 0};
         // a free mailbox (convergent: the drain released it two tiles ago)
         if (MODE == MODE_NN) mbar_wait<!kSplitRegs>(ev_empty(qt & 1), ((uint32_t)(qt >> 1) & 1u) ^ 1u);
+        TLT(t, 2);
         if (MODE == MODE_DUMP) {
           if (dump_item && t < 2) {     // the first 128 rows x 256 columns of the first item
 #pragma unroll
@@ -721,34 +700,109 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
               args.dump[(int64_t)(row_h0 + 8 * ((i >> 1) & 1)) * 256 + col] = a[i];
             }
           }
-        } else {
-          bool any = true;
-          if (MODE == MODE_NN) {
-            // thr is the same in the four lanes of a quad, so the quad's minimum lies inside the window exactly when
-            // some lane's own minimum does: a tile without any such value changes no state and skips the chunk pass.
-            // Masking (partial tile, excluded class) only raises values, so the unmasked minimum decides safely.
-            float m[2] = {kInf, kInf};
+        } else if (MODE == MODE_NN) {
+          // One pass per row and tile.  Value k (0..7) of chunk c of row h sits in a[16 c + 4 (k / 2) + 2 h + k % 2],
+          // column col_base + 32 c + 8 (k / 2) + 2 sub + k % 2.  cm: this lane's minimum of each chunk, per row.
+          auto ai = [](int h, int c, int k) { return 16 * c + 4 * (k >> 1) + 2 * h + (k & 1); };
+          float cm[2][kEvSlots];
 #pragma unroll
-            for (int i = 0; i < 64; i += 4) {
-              m[0] = fminf(m[0], fminf(a[i], a[i + 1]));
-              m[1] = fminf(m[1], fminf(a[i + 2], a[i + 3]));
-            }
-            any = __any_sync(0xffffffffu, (st[0].valid_row && m[0] <= st[0].thr) || (st[1].valid_row && m[1] <= st[1].thr));
-          }
+          for (int h = 0; h < 2; h++)
+#pragma unroll
+            for (int c = 0; c < kEvSlots; c++)
+              cm[h][c] = fminf(fminf(fminf(a[ai(h, c, 0)], a[ai(h, c, 1)]), fminf(a[ai(h, c, 2)], a[ai(h, c, 3)])),
+                               fminf(fminf(a[ai(h, c, 4)], a[ai(h, c, 5)]), fminf(a[ai(h, c, 6)], a[ai(h, c, 7)])));
+          // thr is the same in the four lanes of a quad, so the quad's minimum lies inside the window exactly when
+          // some lane's own minimum does: a tile without any such value changes no state and skips the pass.
+          // Masking (partial tile, excluded class) only raises values, so the unmasked minimum decides safely.
+          bool in[2];
+#pragma unroll
+          for (int h = 0; h < 2; h++)
+            in[h] = st[h].valid_row && fminf(fminf(cm[h][0], cm[h][1]), fminf(cm[h][2], cm[h][3])) <= st[h].thr;
+          const bool any = __any_sync(0xffffffffu, in[0] || in[1]);
+          // timeline slot 3: bit cw = consumer warp cw took the pass on this tile
+          if (any && lane == 0 && args.timeline && blockIdx.x == 0 && tl_tile0 + t < args.timeline_tiles)
+            atomicOr(reinterpret_cast<unsigned long long*>(args.timeline) + (int64_t)(tl_tile0 + t) * 16 + 3,
+                     1ull << cw);
           if (any) {
 #pragma unroll
-            for (int c = 0; c < BN / 32; c++) {
+            for (int h = 0; h < 2; h++)
 #pragma unroll
-              for (int h = 0; h < 2; h++) {
-                float v[8];
+              for (int c = 0; c < kEvSlots; c++) {
+                const int cbase = col_base + 32 * c;
+                if (partial || (EXCL && cbase < st[h].ex_hi && cbase + 32 > st[h].ex_lo)) {
+                  // rare: the chunk runs past the span, or overlaps the train rows this query must ignore.  The
+                  // accumulator is free to overwrite: the next tile's first MMA does not accumulate.
+                  float mn = kInf;
 #pragma unroll
-                for (int jj = 0; jj < 4; jj++) {
-                  v[2 * jj] = a[4 * (4 * c + jj) + 2 * h];
-                  v[2 * jj + 1] = a[4 * (4 * c + jj) + 2 * h + 1];
+                  for (int k = 0; k < 8; k++) {
+                    const int col = cbase + 8 * (k >> 1) + 2 * sub + (k & 1);
+                    if (col >= st[h].col1 || (EXCL && col >= st[h].ex_lo && col < st[h].ex_hi)) a[ai(h, c, k)] = kInf;
+                    mn = fminf(mn, a[ai(h, c, k)]);
+                  }
+                  cm[h][c] = mn;
                 }
-                epi_chunk<MODE, EXCL, RESA>(args, st[h], sh, eb->rec + (row_h0 + 8 * h) * kEvSlots, ev[h], v,
-                                            col_base + 32 * c, c, sub, partial, row_h0 + 8 * h);
               }
+            // the quad's minima of all eight chunks, one batch of independent whole-warp shuffles
+#pragma unroll
+            for (int h = 0; h < 2; h++)
+#pragma unroll
+              for (int c = 0; c < kEvSlots; c++) cm[h][c] = fminf(cm[h][c], __shfl_xor_sync(0xffffffffu, cm[h][c], 1));
+#pragma unroll
+            for (int h = 0; h < 2; h++)
+#pragma unroll
+              for (int c = 0; c < kEvSlots; c++) cm[h][c] = fminf(cm[h][c], __shfl_xor_sync(0xffffffffu, cm[h][c], 2));
+            // the row's running minimum and threshold move once per tile, to the tile's minimum (the same state a
+            // chunk-by-chunk update reaches: that minimum is inside every threshold it would pass through)
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+              EpiState& s = st[h];
+              const float mn = fminf(fminf(cm[h][0], cm[h][1]), fminf(cm[h][2], cm[h][3]));
+              if (s.valid_row && mn <= s.thr && mn < s.best) {
+                s.best = mn;
+                s.s_ref = fminf(s.s_ref, fmaxf(s.best + s.nx, 0.f));
+                s.thr = nn_threshold(s.s_ref, s.nx, s.e2, s.g);
+              }
+            }
+            // events: the chunks inside the row's threshold after the tile (the one the drain applies), each with
+            // the exact mask of its columns inside it, so the re-rank touches only rows inside the window.  Built by
+            // the whole warp: shuffles inside the divergent event branch make ptxas serialise the wgmma.
+            uint32_t mk[2][kEvSlots];
+#pragma unroll
+            for (int h = 0; h < 2; h++)
+#pragma unroll
+              for (int c = 0; c < kEvSlots; c++) {
+                mk[h][c] = 0;
+#pragma unroll
+                for (int k = 0; k < 8; k++)
+                  mk[h][c] |= (a[ai(h, c, k)] <= st[h].thr) ? (1u << (8 * (k >> 1) + 2 * sub + (k & 1))) : 0u;
+              }
+#pragma unroll
+            for (int h = 0; h < 2; h++)
+#pragma unroll
+              for (int c = 0; c < kEvSlots; c++) mk[h][c] |= __shfl_xor_sync(0xffffffffu, mk[h][c], 1);
+#pragma unroll
+            for (int h = 0; h < 2; h++)
+#pragma unroll
+              for (int c = 0; c < kEvSlots; c++) {
+                mk[h][c] |= __shfl_xor_sync(0xffffffffu, mk[h][c], 2);
+                if (st[h].valid_row && cm[h][c] <= st[h].thr && cm[h][c] < kInf) {
+                  ev[h] |= 1 << c;
+                  if (sub == 0) eb->rec[(row_h0 + 8 * h) * kEvSlots + c] = EvRecord{col_base + 32 * c, mk[h][c], cm[h][c], st[h].thr};
+                }
+              }
+          }
+        } else {
+#pragma unroll
+          for (int c = 0; c < BN / 32; c++) {
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+              float v[8];
+#pragma unroll
+              for (int jj = 0; jj < 4; jj++) {
+                v[2 * jj] = a[4 * (4 * c + jj) + 2 * h];
+                v[2 * jj + 1] = a[4 * (4 * c + jj) + 2 * h + 1];
+              }
+              epi_chunk<MODE, EXCL>(args, st[h], sh, v, col_base + 32 * c, sub, partial, row_h0 + 8 * h);
             }
           }
         }
@@ -845,9 +899,7 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
                   v[2 * jj] = acc[4 * (4 * c + jj) + 2 * h];
                   v[2 * jj + 1] = acc[4 * (4 * c + jj) + 2 * h + 1];
                 }
-                int ev = 0;
-                epi_chunk<MODE, EXCL, RESA>(args, st[h], sh, nullptr, ev, v, col_base + 32 * c, c, sub, partial,
-                                            row_h0 + 8 * h);
+                epi_chunk<MODE, EXCL>(args, st[h], sh, v, col_base + 32 * c, sub, partial, row_h0 + 8 * h);
               }
             }
           }

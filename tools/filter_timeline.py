@@ -13,7 +13,10 @@ Runs C2's stage-1 (same-class columns) and stage-2 (other-class columns) searche
   lead     producer ahead of the consumers: producer starts loading the tile (slot 8) -> consumer starts
            issuing it (slot 0); large means the ring is full and the consumers are the limit
   load     producer: first -> last TMA issue of the tile (slot 8 -> slot 10), including waits for free stages
-p50 / p90 over the tiles of block 0.  Stage 2 runs here from freshly packed queries, so its running minima start
+  ev_wait  consumer: the epilogue's wait for a free event mailbox (slot 1 -> slot 2), i.e. for the drain to have
+           taken the events of two tiles back; part of `epilogue`
+p50 / p90 over the tiles of block 0.  `chunk_pass` is, per consumer warp, the share of block 0's tiles on which the
+warp took the chunk pass (some row's tile minimum inside its window; slot 3 holds one bit per warp).  Stage 2 runs here from freshly packed queries, so its running minima start
 at +inf; bench.py's stage 2 starts from the bounds stage 1 found, so fewer of its tiles reach the event path.
 `search_ms` times the whole search call (query packing, the filter launch, the re-rank), not the filter alone.
 `--root` runs the package found in another tree (e.g. a build of an earlier commit), so that two versions can be
@@ -67,12 +70,17 @@ def main():
         t = t[(t[:, 0] > 0) & (t[:, 1] > 0) & (t[:, 7] > 0) & (t[:, 8] > 0) & (t[:, 10] > 0)]
         ph = {"mma": t[:, 1] - t[:, 0], "epilogue": t[:, 7] - t[:, 1], "period": np.diff(t[:, 0]),
               "lead": t[:, 0] - t[:, 8], "load": t[:, 10] - t[:, 8]}
+        ph["ev_wait"] = (t[:, 2] - t[:, 1])[t[:, 2] > 0]
         d = buf.cpu().numpy()
         d = d[(d[:, 11] > 0) & (d[:, 12] > 0)]
         ph["drain"] = d[:, 12] - d[:, 11]
         rec = {"tiles": int(len(t)), "search_ms": ev0.elapsed_time(ev1)}
         for k, v in ph.items():
             rec[k] = {"p50": float(np.percentile(v, 50)), "p90": float(np.percentile(v, 90))} if len(v) else None
+        q_rows, t_rows = C.c_int32(), C.c_int32()
+        lib.tip_nn_filter_tile(128, C.byref(q_rows), C.byref(t_rows))
+        warps = q_rows.value // 16          # one consumer warp per 16 query rows of a tile
+        rec["chunk_pass"] = [round(float(((t[:, 3] >> w) & 1).mean()), 3) for w in range(warps)] if len(t) else None
         out[name] = rec
         print(name, json.dumps(rec), flush=True)
     if args.json:
