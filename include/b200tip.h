@@ -17,6 +17,7 @@
  *   tip_vote_add        handler_model.py:148-166 uwiz VariationRatio: argmax votes of MC-dropout samples,
  *   tip_vote_finish     streamed pass by pass; mode and 1 - votes / samples
  *   tip_kmnc            src/core/neuron_coverage.py:82-94 (+ sum_score :8-22)
+ *   tip_kmnc_packed     the same profile bit-packed in HBM, for tip_cam_bits
  *   tip_cam_buckets     src/core/prioritizers.py:16-45 (greedy loop of cam) on compact KMNC profiles
  *   tip_pair_prep       (new) operand packing for the tensor-core pass
  *   tip_nn_filter       src/core/surprise.py:638-647   the B x M x D difference/norm/min, as a
@@ -142,6 +143,15 @@ int tip_vote_finish(const int32_t* counts, int64_t n, int64_t c, int64_t samples
 int tip_kmnc(const void* act, int act_dtype, int64_t n, int64_t d, const void* mins,
              const void* jumps, int stat_dtype, int32_t sections, void* bucket, int bucket_dtype,
              int32_t* score, void* stream);
+/* The same sections, bit-packed for tip_cam_bits (the reference's dense n x d x sections profile,
+ * plane by plane): bits[n * sections * W] with W = tip_cover_packed_words(d).  Row r holds `sections`
+ * planes of W words; in plane s, bit l of word 4g + i is set when neuron 128g + 4l + i lies in section
+ * s — the layout of tip_cover_threshold (one plane: NAC's, two: NBC's plane order).  Padding bits are
+ * 0; every word of a row is written.  score[n] as tip_kmnc.  Section membership is tip_kmnc's
+ * arithmetic, so the bits are set exactly where tip_kmnc's bucket ids say. */
+int tip_kmnc_packed(const void* act, int act_dtype, int64_t n, int64_t d, const void* mins,
+                    const void* jumps, int stat_dtype, int32_t sections, uint32_t* bits, int32_t* score,
+                    void* stream);
 
 /* ---- Coverage-Additional Method over compact coverage profiles (prioritizers.py:16-59) ----
  * bucket: n x d section ids as tip_kmnc writes them (TIP_I16 / TIP_I32, -1 = none): the one-hot-per-

@@ -49,6 +49,7 @@ _SIGNATURES = {
     "tip_vote_add": (C.c_int, [_vp, C.c_int, _i64, _i64, _i64, _i64, _i64, _vp, _vp]),
     "tip_vote_finish": (C.c_int, [_vp, _i64, _i64, _i64, _vp, _vp, _vp]),
     "tip_kmnc": (C.c_int, [_vp, C.c_int, _i64, _i64, _vp, _vp, C.c_int, _i32, _vp, C.c_int, _vp, _vp]),
+    "tip_kmnc_packed": (C.c_int, [_vp, C.c_int, _i64, _i64, _vp, _vp, C.c_int, _i32, _vp, _vp, _vp]),
     "tip_cam_buckets": (C.c_int, [_vp, C.c_int, _i64, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _vp]),
     "tip_sc_cam": (C.c_int, [_vp, C.c_int, _i64, _vp, _i32, _vp, _vp, _vp, _vp]),
     "tip_cover_packed_words": (_i64, [_i64]),

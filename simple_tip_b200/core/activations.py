@@ -97,6 +97,33 @@ class TransparentModel:
         return [torch.cat(lst, dim=0) for lst in per_layer]
 
 
+class HookedModelHandler:
+    """What the study's arms for a torch model share (`SurpriseHandler`, `CoverageWorker`): the hooked model in
+    `self.base_model` (a `TransparentModel`), the device it runs on, and timers that include the device work."""
+
+    base_model: TransparentModel
+
+    def _model_device(self):
+        import torch
+
+        return next(iter(self.base_model.model.parameters()), torch.empty(0)).device
+
+    def _synced(self, fn, timer):
+        """fn() timed by `timer`, which stops after a synchronise of the current CUDA device (the scoring device)
+        and of the model's device when that is another CUDA device."""
+        import torch
+
+        from .. import engine as E
+
+        score_dev, model_dev = E.require_cuda(), self._model_device()
+        with timer:
+            res = fn()
+            torch.cuda.synchronize(score_dev)
+            if model_dev.type == "cuda" and model_dev != score_dev:
+                torch.cuda.synchronize(model_dev)
+        return res
+
+
 DROPOUT_SAMPLE_SIZE = 200      # handler_model.py:7
 MC_ROWS_PER_PASS = 8192        # rows of one MC-dropout forward pass: a batch is replicated up to this many
 

@@ -6,7 +6,7 @@ pass computes, per (sample, neuron), the section index i with
 rounding) and the per-sample count, i.e. the compact form of the reference's dense
 N x D x sections boolean profile.  `KMNC.__call__` expands it to the dense profile only because
 the reference API returns one (consumers: `cam`, handler_coverage.py:122-124); `buckets()` is the
-compact entry point for large `sections`.  NAC / NBC / SNAC / TKNC (neuron_coverage.py:52-62,97-173)
+compact entry point for large `sections`, `packed()` the same sections bit-packed in HBM (one plane per section).  NAC / NBC / SNAC / TKNC (neuron_coverage.py:52-62,97-173)
 run on the GPU as well (csrc/coverage.cu): the boundaries are the reference's NumPy expressions, the
 comparisons happen in NumPy's promoted dtype, so scores and profiles are bit-identical; every class
 also offers `packed(...)`, the same profile bit-packed in HBM for `prioritizers.cam_from_bits`.
@@ -174,24 +174,21 @@ class KMNC(CoverageMethod):
         lo = self._lo
         return [lo + self._jumps * i for i in range(self.sections + 1)]
 
-    def buckets(self, activations, device_out: bool = False):
-        """(scores [N] in the reference's score dtype — int32 CUDA tensor with device_out —, bucket ids [N, D] int16/int32;
-        -1 = no section covered).
-        Activations may be NumPy arrays or device-resident torch tensors (one or a list);
-        device_out=True returns the two results as CUDA tensors (no D2H of the N x D bucket ids)."""
+    def _prepare(self, activations):
+        """(activations as one [N, D] matrix — a contiguous CUDA tensor, or a NumPy array still on the host —, whether
+        it came from the device, its NumPy dtype, the statistics' dtype)"""
         import torch
 
-        from .. import _lib
         from .. import engine as E
 
         dev_act = E.device_matrix(activations)
         if dev_act is not None:
             act = dev_act if dev_act.dtype in (torch.float32, torch.float64) else dev_act.to(torch.float32)
             act = act.contiguous()
-        elif isinstance(activations, np.ndarray):
-            act = activations.reshape((activations.shape[0], -1))
+        elif isinstance(activations, np.ndarray):   # (explicit widths: a -1 cannot be resolved for 0 samples)
+            act = activations.reshape((activations.shape[0], int(np.prod(activations.shape[1:]))))
         elif len(activations) == 1:          # one layer: no concatenation copy (keeps a pinned buffer pinned)
-            act = np.reshape(activations[0], (activations[0].shape[0], -1))
+            act = np.reshape(activations[0], (activations[0].shape[0], int(np.prod(activations[0].shape[1:]))))
         else:
             act = flatten_layers(activations)
         stat_dt = self._jumps.dtype
@@ -202,13 +199,31 @@ class KMNC(CoverageMethod):
             if act.dtype not in (np.float32, np.float64):
                 raise TypeError(f"unsupported activation dtype {act.dtype}")
         act_np_dtype = E.NP_DTYPE[act.dtype] if dev_act is not None else act.dtype
+        assert act.shape[1] == self._lo.shape[0], "activation width does not match the min/max statistics"
+        return act, dev_act is not None, act_np_dtype, stat_dt
+
+    def _device_stats(self, dev):
+        from .. import engine as E
+
+        if self._dev_stats is None:
+            self._dev_stats = (E.to_device(self._lo.astype(self._jumps.dtype), dev), E.to_device(self._jumps, dev))
+        return self._dev_stats
+
+    def buckets(self, activations, device_out: bool = False):
+        """(scores [N] in the reference's score dtype — int32 CUDA tensor with device_out —, bucket ids [N, D] int16/int32;
+        -1 = no section covered).
+        Activations may be NumPy arrays or device-resident torch tensors (one or a list);
+        device_out=True returns the two results as CUDA tensors (no D2H of the N x D bucket ids)."""
+        import torch
+
+        from .. import _lib
+        from .. import engine as E
+
+        act, on_device, act_np_dtype, stat_dt = self._prepare(activations)
         dev = E.require_cuda()
         lib = _lib.load()
         n, d = act.shape
-        assert d == self._lo.shape[0], "activation width does not match the min/max statistics"
-        if self._dev_stats is None:
-            self._dev_stats = (E.to_device(self._lo.astype(stat_dt), dev), E.to_device(self._jumps, dev))
-        lo_dev, jump_dev = self._dev_stats
+        lo_dev, jump_dev = self._device_stats(dev)
         small = self.sections <= np.iinfo(np.int16).max
         bdt, btag = (torch.int16, _lib.TIP_I16) if small else (torch.int32, _lib.TIP_I32)
 
@@ -217,7 +232,7 @@ class KMNC(CoverageMethod):
                                     E.tip_dtype(stat_dt), self.sections, E._p(bucket_chunk), btag, E._p(score_chunk),
                                     E._stream()), "tip_kmnc")
 
-        if device_out or dev_act is not None or n * d * act.dtype.itemsize < self.PIPELINE_BYTES:
+        if device_out or on_device or n * d * act.dtype.itemsize < self.PIPELINE_BYTES:
             a_dev = E.to_device(act, dev)
             bucket = torch.empty((n, d), dtype=bdt, device=dev)
             score = torch.empty(n, dtype=torch.int32, device=dev)
@@ -282,6 +297,38 @@ class KMNC(CoverageMethod):
             j.result()
         main.wait_stream(up)
         return hs.numpy().astype(_score_dtype(d * self.sections)), out
+
+    def packed(self, activations):
+        """(scores int32 [N], profile bit-packed [N, sections * W] int32) as CUDA tensors — nothing leaves HBM; feed
+        to `prioritizers.cam_from_bits`.  W = `tip_cover_packed_words(D)`; plane s holds section s in NAC's layout
+        (libb200tip `tip_kmnc_packed`), and the scores are those of `buckets()`.  Takes what `buckets()` takes.
+
+        The bits take N * sections * W * 4 bytes of HBM (W = 4 * ceil(D / 128)): 91 MB for N = 10 k, D = 36 k and two
+        sections, where `buckets()`' int16 ids take 728 MB.  A row of sections * W >= 2^31 words is beyond
+        `cam_from_bits` (ValueError before any launch); that many sections stay with `buckets()` / `cam_from_buckets`."""
+        import torch
+
+        from .. import _lib
+        from .. import engine as E
+
+        act, _, act_np_dtype, stat_dt = self._prepare(activations)
+        lib = _lib.load()
+        n, d = act.shape
+        words = self.sections * int(lib.tip_cover_packed_words(d))
+        if words >= 2 ** 31:
+            raise ValueError(f"KMNC.packed: {self.sections} sections x {words // self.sections} words per row exceed "
+                             "cam_from_bits' 2^31 words; use buckets() and cam_from_buckets")
+        dev = E.require_cuda()
+        bits = torch.empty((n, words), dtype=torch.int32, device=dev)
+        score = torch.empty(n, dtype=torch.int32, device=dev)
+        if n == 0:
+            return score, bits
+        a_dev = E.to_device(act, dev)
+        lo_dev, jump_dev = self._device_stats(dev)
+        _lib.check(lib.tip_kmnc_packed(E._p(a_dev), E.tip_dtype(act_np_dtype), n, d, E._p(lo_dev), E._p(jump_dev),
+                                       E.tip_dtype(stat_dt), self.sections, E._p(bits), E._p(score), E._stream()),
+                   "tip_kmnc_packed")
+        return score, bits
 
     PIPELINE_BYTES = 32 << 20
     PIPELINE_CHUNKS = 8

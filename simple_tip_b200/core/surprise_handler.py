@@ -11,7 +11,7 @@ from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 
-from .activations import TransparentModel
+from .activations import HookedModelHandler, TransparentModel
 from .prioritizers import cam_from_surprise
 from .surprise import DSA, LSA, MDSA, MLSA, MultiModalSA, SurpriseCoverageMapper
 from .timer import Timer
@@ -19,7 +19,7 @@ from .timer import Timer
 NUM_SC_BUCKETS = 1000          # handler_surprise.py:14
 
 
-class SurpriseHandler:
+class SurpriseHandler(HookedModelHandler):
     """`SurpriseHandler(model, sa_layers, training_data)` + `evaluate_all(datasets)` of handler_surprise.py for a
     `torch.nn.Module` whose last output is its softmax.
 
@@ -58,24 +58,6 @@ class SurpriseHandler:
         self.train_at_timer = Timer()
         self.train_ats, self.train_pred = self._synced(lambda: self._acti_and_pred(training_data),
                                                        self.train_at_timer)
-
-    def _model_device(self):
-        import torch
-
-        return next(iter(self.base_model.model.parameters()), torch.empty(0)).device
-
-    def _synced(self, fn, timer: Timer):
-        import torch
-
-        from .. import engine as E
-
-        score_dev, model_dev = E.require_cuda(), self._model_device()
-        with timer:
-            res = fn()
-            torch.cuda.synchronize(score_dev)
-            if model_dev.type == "cuda" and model_dev != score_dev:
-                torch.cuda.synchronize(model_dev)
-        return res
 
     def _acti_and_pred(self, data) -> Tuple[List, np.ndarray]:
         """handler_surprise.py:51-57: the hooked layers and the predictions of one forward pass."""

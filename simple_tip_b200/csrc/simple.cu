@@ -419,19 +419,36 @@ __device__ __forceinline__ int kmnc_bucket_ff(float a, float lo, float jump, int
   return kmnc_bucket_slow(a, lo, jump, k);
 }
 
+// Output of the KMNC kernels: bucket ids (TB = int16_t / int32_t, n x d), or with TB = uint32_t the profile
+// bit-packed as tip_kmnc_packed documents it (n rows of k planes of kmnc_words(d) words).
+template <typename TB> struct KmncBits { static constexpr bool value = false; };
+template <> struct KmncBits<uint32_t> { static constexpr bool value = true; };
+
+__host__ __device__ inline int64_t kmnc_words(int64_t d) { return 4 * ((d + 127) / 128); }   // tip_cover_packed_words
+
+// bits of one row + plane: neuron c lies in word 4 * (c / 128) + c % 4, bit (c % 128) / 4
+__device__ __forceinline__ void kmnc_or_bit(uint32_t* plane, int64_t c) {
+  atomicOr(plane + 4 * (c / 128) + (c % 4), 1u << ((c % 128) / 4));
+}
+
 template <typename TA, typename TS, typename TB>
 __global__ void __launch_bounds__(256) kmnc_kernel(const TA* __restrict__ act, int64_t n, int64_t d,
                                                    const TS* __restrict__ mins, const TS* __restrict__ jumps,
                                                    int k, TB* __restrict__ bucket, int32_t* __restrict__ score) {
+  constexpr bool kBits = KmncBits<TB>::value;   // bucket: zero-filled packed words, set bit by bit
   __shared__ int warp_cnt[8];
   for (int64_t row = blockIdx.x; row < n; row += gridDim.x) {
     const TA* a = act + row * d;
-    TB* b = bucket ? bucket + row * d : nullptr;
+    TB* b = bucket ? bucket + row * (kBits ? k * kmnc_words(d) : d) : nullptr;
     int cnt = 0;
     for (int64_t j = threadIdx.x; j < d; j += 256) {
       const int i = kmnc_bucket<TA, TS>(a[j], mins[j], jumps[j], k);
       cnt += (i >= 0);
-      if (b) b[j] = (TB)i;
+      if constexpr (kBits) {
+        if (i >= 0) kmnc_or_bit(b + i * kmnc_words(d), j);
+      } else {
+        if (b) b[j] = (TB)i;
+      }
     }
     cnt = warp_sum(cnt);
     if ((threadIdx.x & 31) == 0) warp_cnt[threadIdx.x >> 5] = cnt;
@@ -448,11 +465,14 @@ __global__ void __launch_bounds__(256) kmnc_kernel(const TA* __restrict__ act, i
 // float traces, float statistics, d % 4 == 0, 16-byte aligned: 128-bit loads, 64-bit stores.
 // One warp owns 128 consecutive neurons of one sample at a time (grid-stride over such chunks);
 // per-sample counts are accumulated with one atomic per chunk into a zeroed score array.
+// Packed bits (TB = uint32_t): such a chunk is exactly one group of 128 neurons, so per plane four ballots
+// make its four words, which lane 0 stores as one 16-byte word.
 template <typename TB>
 __global__ void __launch_bounds__(256) kmnc_vec4_kernel(const float* __restrict__ act, int64_t n, int64_t d,
                                                         const float* __restrict__ mins,
                                                         const float* __restrict__ jumps, int k,
                                                         TB* __restrict__ bucket, int32_t* __restrict__ score) {
+  constexpr bool kBits = KmncBits<TB>::value;
   const int lane = threadIdx.x & 31;
   const int64_t d4 = d >> 2;
   const int64_t cpr = (d4 + 31) >> 5;  // chunks per row
@@ -480,6 +500,7 @@ __global__ void __launch_bounds__(256) kmnc_vec4_kernel(const float* __restrict_
 #pragma unroll
     for (int u = 0; u < kUnroll; u++) {
       int cnt = 0;
+      int4 sec = make_int4(-1, -1, -1, -1);   // (packed bits only)
       if (ok[u]) {
         const float4 lo = __ldg(reinterpret_cast<const float4*>(mins) + j[u]);
         const float4 jp = __ldg(reinterpret_cast<const float4*>(jumps) + j[u]);
@@ -488,7 +509,9 @@ __global__ void __launch_bounds__(256) kmnc_vec4_kernel(const float* __restrict_
         const int i2 = kmnc_bucket_ff(v[u].z, lo.z, jp.z, k);
         const int i3 = kmnc_bucket_ff(v[u].w, lo.w, jp.w, k);
         cnt = (i0 >= 0) + (i1 >= 0) + (i2 >= 0) + (i3 >= 0);
-        if (bucket) {
+        if constexpr (kBits) {
+          sec = make_int4(i0, i1, i2, i3);
+        } else if (bucket) {
           TB* bp = bucket + row[u] * d + (j[u] << 2);
           if (sizeof(TB) == 2) {
             *reinterpret_cast<short4*>(bp) = make_short4((short)i0, (short)i1, (short)i2, (short)i3);
@@ -498,6 +521,15 @@ __global__ void __launch_bounds__(256) kmnc_vec4_kernel(const float* __restrict_
         }
       }
       if (chunk0 + (int64_t)u * nwarps < total) {   // warp-uniform
+        if constexpr (kBits) {
+          const int64_t words = kmnc_words(d);
+          uint4* dst = reinterpret_cast<uint4*>(bucket + row[u] * k * words) + (j[u] >> 5);   // group (j - lane) / 32
+          for (int s = 0; s < k; s++) {
+            const uint4 w = make_uint4(__ballot_sync(0xffffffffu, sec.x == s), __ballot_sync(0xffffffffu, sec.y == s),
+                                       __ballot_sync(0xffffffffu, sec.z == s), __ballot_sync(0xffffffffu, sec.w == s));
+            if (lane == 0) dst[s * (words >> 2)] = w;
+          }
+        }
         cnt = warp_sum(cnt);
         if (lane == 0 && cnt) atomicAdd(score + row[u], cnt);
       }
@@ -570,12 +602,13 @@ __device__ __forceinline__ void red_add_s32_if(int32_t* p, int v, bool on) {   /
                : "memory");
 }
 
-// one sample row x four neurons of this thread: sections, optional store, number of covered neurons
+// one sample row x four neurons of this thread: sections (also into `sec`), optional store of bucket ids,
+// number of covered neurons
 template <typename TB, bool STORE>
 __device__ __forceinline__ int kmnc_strip_row(const float4 v, const KmncLane& s0, const KmncLane& s1,
                                               const KmncLane& s2, const KmncLane& s3, int k,
                                               const float* __restrict__ lo_g, const float* __restrict__ jp_g,
-                                              TB* __restrict__ bp) {
+                                              TB* __restrict__ bp, int4& sec) {
   bool ok0, ok1, ok2, ok3;
   int i0 = kmnc_fast(v.x, s0, ok0);
   int i1 = kmnc_fast(v.y, s1, ok1);
@@ -587,7 +620,8 @@ __device__ __forceinline__ int kmnc_strip_row(const float4 v, const KmncLane& s0
     if (!ok2) i2 = kmnc_bucket_slow(v.z, __ldg(lo_g + 2), __ldg(jp_g + 2), k);
     if (!ok3) i3 = kmnc_bucket_slow(v.w, __ldg(lo_g + 3), __ldg(jp_g + 3), k);
   }
-  if (STORE) {
+  sec = make_int4(i0, i1, i2, i3);
+  if (STORE && !KmncBits<TB>::value) {
     if (sizeof(TB) == 2) {
       *reinterpret_cast<short4*>(bp) = make_short4((short)i0, (short)i1, (short)i2, (short)i3);
     } else {
@@ -605,18 +639,33 @@ __device__ __forceinline__ float4 ld_stream_f4(const float4* p) {
   return v;
 }
 
+// dst: bucket ids, row pitch d; or (TB = uint32_t) this warp's four words in plane 0 of the packed profile, row
+// pitch k planes of `words`: per plane four ballots under `live` (the lanes past d contribute 0 bits), one
+// 16-byte store by the leader.
 template <typename TB, bool STORE, int ROWS>
 __device__ __forceinline__ void kmnc_strip_batch(const float4* __restrict__ src, int64_t d4, int64_t d,
                                                  const KmncLane& s0, const KmncLane& s1, const KmncLane& s2,
                                                  const KmncLane& s3, int k, const float* __restrict__ lo_g,
                                                  const float* __restrict__ jp_g, TB* __restrict__ dst,
                                                  int32_t* __restrict__ sc, unsigned live, bool leader) {
+  constexpr bool kBits = KmncBits<TB>::value;
   float4 v[ROWS];
 #pragma unroll
   for (int u = 0; u < ROWS; u++) v[u] = ld_stream_f4(src + u * d4);
 #pragma unroll
   for (int u = 0; u < ROWS; u++) {
-    int cnt = kmnc_strip_row<TB, STORE>(v[u], s0, s1, s2, s3, k, lo_g, jp_g, STORE ? dst + u * d : nullptr);
+    int4 sec;
+    int cnt = kmnc_strip_row<TB, STORE>(v[u], s0, s1, s2, s3, k, lo_g, jp_g,
+                                        STORE && !kBits ? dst + u * d : nullptr, sec);
+    if constexpr (kBits) {
+      const int64_t words = kmnc_words(d);
+      uint4* row = reinterpret_cast<uint4*>(dst + u * k * words);
+      for (int s = 0; s < k; s++) {
+        const uint4 w = make_uint4(__ballot_sync(live, sec.x == s), __ballot_sync(live, sec.y == s),
+                                   __ballot_sync(live, sec.z == s), __ballot_sync(live, sec.w == s));
+        if (leader) row[s * (words >> 2)] = w;
+      }
+    }
     cnt = __reduce_add_sync(live, cnt);
     red_add_s32_if(sc + u, cnt, leader);
   }
@@ -646,43 +695,92 @@ __global__ void __launch_bounds__(256) kmnc_strip_kernel(const float* __restrict
   const int64_t row0 = n * l / lanes;
   const int64_t row1 = n * (l + 1) / lanes;
   const float4* src = reinterpret_cast<const float4*>(act) + row0 * d4 + j;
-  TB* dst = STORE ? bucket + row0 * d + (j << 2) : nullptr;
+  // packed bits: a warp owns exactly the 128 neurons of group j / 32, i.e. words 4 * (j / 32) .. + 3 of each plane
+  const int64_t pitch = KmncBits<TB>::value ? k * kmnc_words(d) : d;
+  TB* dst = STORE ? bucket + row0 * pitch + (KmncBits<TB>::value ? 4 * (j >> 5) : (j << 2)) : nullptr;
   int32_t* sc = score + row0;
   int64_t r = row0;
   for (; r + kStripRows <= row1; r += kStripRows) {
     kmnc_strip_batch<TB, STORE, kStripRows>(src, d4, d, s0, s1, s2, s3, k, lo_g, jp_g, dst, sc, live, leader);
     src += kStripRows * d4;
-    if (STORE) dst += kStripRows * d;
+    if (STORE) dst += kStripRows * pitch;
     sc += kStripRows;
   }
   if (r + 4 <= row1) {
     kmnc_strip_batch<TB, STORE, 4>(src, d4, d, s0, s1, s2, s3, k, lo_g, jp_g, dst, sc, live, leader);
     src += 4 * d4;
-    if (STORE) dst += 4 * d;
+    if (STORE) dst += 4 * pitch;
     sc += 4;
     r += 4;
   }
   for (; r < row1; r++) {
     kmnc_strip_batch<TB, STORE, 1>(src, d4, d, s0, s1, s2, s3, k, lo_g, jp_g, dst, sc, live, leader);
     src += d4;
-    if (STORE) dst += d;
+    if (STORE) dst += pitch;
     sc++;
   }
 }
 
-template <typename TA, typename TS>
+// the generic kernel: any dtypes, any alignment; packed bits are OR-ed into a zero-filled buffer
+template <typename TA, typename TS, typename TB>
 static int launch_kmnc(const void* act, int64_t n, int64_t d, const void* mins, const void* jumps, int k,
-                       void* bucket, int bucket_dtype, int32_t* score, cudaStream_t st) {
+                       TB* out, int32_t* score, cudaStream_t st) {
+  if (KmncBits<TB>::value)
+    TIP_CHECK_CUDA(cudaMemsetAsync(out, 0, (size_t)n * k * kmnc_words(d) * sizeof(uint32_t), st));
   const int grid = (int)std::min<int64_t>(n, (int64_t)sm_count() * 8);
-  if (bucket == nullptr || bucket_dtype == TIP_I16) {
-    kmnc_kernel<TA, TS, int16_t><<<grid, 256, 0, st>>>((const TA*)act, n, d, (const TS*)mins, (const TS*)jumps,
-                                                       k, (int16_t*)bucket, score);
-  } else {
-    kmnc_kernel<TA, TS, int32_t><<<grid, 256, 0, st>>>((const TA*)act, n, d, (const TS*)mins, (const TS*)jumps,
-                                                       k, (int32_t*)bucket, score);
-  }
+  kmnc_kernel<TA, TS, TB><<<grid, 256, 0, st>>>((const TA*)act, n, d, (const TS*)mins, (const TS*)jumps, k, out, score);
   TIP_LAUNCH_CHECK();
   return TIP_OK;
+}
+
+// Routes one KMNC call (n >= 1) to its kernel: float traces and statistics, d % 4 == 0 and 16-byte aligned take
+// the column-strip kernel (many samples) or the vec4 kernel (few); everything else the generic kernel.
+// out: bucket ids of TB (nullptr with STORE = false: scores only), or the packed profile (TB = uint32_t).
+template <typename TB, bool STORE>
+static int kmnc_route(const void* act, int act_dtype, int64_t n, int64_t d, const void* mins, const void* jumps,
+                      int stat_dtype, int32_t sections, TB* out, int32_t* score, cudaStream_t st) {
+  if (act_dtype == TIP_F32 && stat_dtype == TIP_F32) {
+    const bool aligned = (d % 4 == 0) && (((uintptr_t)act | (uintptr_t)mins | (uintptr_t)jumps) & 15) == 0 &&
+                         (out == nullptr || ((uintptr_t)out & 15) == 0);
+    if (aligned) {
+      TIP_CHECK_CUDA(cudaMemsetAsync(score, 0, (size_t)n * sizeof(int32_t), st));
+      const int64_t nstrips = ((d >> 2) + 255) / 256;
+      if (n >= 4 * kStripRows && nstrips <= 65535 && sections <= (1 << 22)) {
+        // enough samples to amortise the per-block statistics load: column-strip kernel, one resident wave
+        const void* fn = (const void*)kmnc_strip_kernel<TB, STORE>;
+        static int per_sm = 0;   // occupancy of this instance (same on every device of a box)
+        if (per_sm == 0) {
+          int v = 0;
+          TIP_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, fn, 256, 0));
+          per_sm = std::max(v, 1);
+        }
+        const int64_t resident = (int64_t)sm_count() * per_sm;
+        const int64_t lanes = std::max<int64_t>(1, std::min<int64_t>(resident / nstrips, n / (2 * kStripRows)));
+        const int ns = (int)nstrips, ln = (int)lanes;
+        const float* a = (const float*)act;
+        const float* lo = (const float*)mins;
+        const float* jp = (const float*)jumps;
+        void* args[] = {&a, &n, &d, &lo, &jp, &sections, &out, &score, (void*)&ns, (void*)&ln};
+        TIP_CHECK_CUDA(cudaLaunchKernel(fn, dim3((unsigned)(nstrips * lanes)), dim3(256), args, 0, st));
+        TIP_LAUNCH_CHECK();
+        return TIP_OK;
+      }
+      const int64_t chunks = n * (((d >> 2) + 31) >> 5);
+      const int grid = (int)std::min<int64_t>((chunks + 7) / 8, (int64_t)sm_count() * 8);
+      kmnc_vec4_kernel<TB><<<grid, 256, 0, st>>>((const float*)act, n, d, (const float*)mins, (const float*)jumps,
+                                                 sections, out, score);
+      TIP_LAUNCH_CHECK();
+      return TIP_OK;
+    }
+    return launch_kmnc<float, float>(act, n, d, mins, jumps, sections, out, score, st);
+  }
+  if (act_dtype == TIP_F32 && stat_dtype == TIP_F64)
+    return launch_kmnc<float, double>(act, n, d, mins, jumps, sections, out, score, st);
+  if (act_dtype == TIP_F64 && stat_dtype == TIP_F32)
+    return launch_kmnc<double, float>(act, n, d, mins, jumps, sections, out, score, st);
+  if (act_dtype == TIP_F64 && stat_dtype == TIP_F64)
+    return launch_kmnc<double, double>(act, n, d, mins, jumps, sections, out, score, st);
+  TIP_REQUIRE(false, "dtypes must be TIP_F32 / TIP_F64");
 }
 
 // =============================================================================================
@@ -1041,56 +1139,24 @@ extern "C" int tip_kmnc(const void* act, int act_dtype, int64_t n, int64_t d, co
   TIP_REQUIRE(!(bucket && bucket_dtype == TIP_I16) || sections <= 32767, "sections exceed int16 bucket ids");
   if (n == 0) return TIP_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  if (act_dtype == TIP_F32 && stat_dtype == TIP_F32) {
-    const bool aligned = (d % 4 == 0) && (((uintptr_t)act | (uintptr_t)mins | (uintptr_t)jumps) & 15) == 0 &&
-                         (bucket == nullptr || ((uintptr_t)bucket & 15) == 0);
-    if (aligned) {
-      TIP_CHECK_CUDA(cudaMemsetAsync(score, 0, (size_t)n * sizeof(int32_t), st));
-      const int64_t nstrips = ((d >> 2) + 255) / 256;
-      if (n >= 4 * kStripRows && nstrips <= 65535 && sections <= (1 << 22)) {
-        // enough samples to amortise the per-block statistics load: column-strip kernel, one resident wave
-        const bool i16 = bucket == nullptr || bucket_dtype == TIP_I16;
-        const void* fn = bucket == nullptr ? (const void*)kmnc_strip_kernel<int16_t, false>
-                         : i16             ? (const void*)kmnc_strip_kernel<int16_t, true>
-                                           : (const void*)kmnc_strip_kernel<int32_t, true>;
-        const int which = bucket == nullptr ? 0 : (i16 ? 1 : 2);
-        static int per_sm_of[3] = {0, 0, 0};   // occupancy of each instance (same on every device of a box)
-        if (per_sm_of[which] == 0) {
-          int v = 0;
-          TIP_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, fn, 256, 0));
-          per_sm_of[which] = std::max(v, 1);
-        }
-        const int64_t resident = (int64_t)sm_count() * per_sm_of[which];
-        const int64_t lanes = std::max<int64_t>(1, std::min<int64_t>(resident / nstrips, n / (2 * kStripRows)));
-        const int ns = (int)nstrips, ln = (int)lanes;
-        const float* a = (const float*)act;
-        const float* lo = (const float*)mins;
-        const float* jp = (const float*)jumps;
-        void* args[] = {&a, &n, &d, &lo, &jp, &sections, &bucket, &score, (void*)&ns, (void*)&ln};
-        TIP_CHECK_CUDA(cudaLaunchKernel(fn, dim3((unsigned)(nstrips * lanes)), dim3(256), args, 0, st));
-        TIP_LAUNCH_CHECK();
-        return TIP_OK;
-      }
-      const int64_t chunks = n * (((d >> 2) + 31) >> 5);
-      const int grid = (int)std::min<int64_t>((chunks + 7) / 8, (int64_t)sm_count() * 8);
-      if (bucket == nullptr || bucket_dtype == TIP_I16)
-        kmnc_vec4_kernel<int16_t><<<grid, 256, 0, st>>>((const float*)act, n, d, (const float*)mins,
-                                                        (const float*)jumps, sections, (int16_t*)bucket, score);
-      else
-        kmnc_vec4_kernel<int32_t><<<grid, 256, 0, st>>>((const float*)act, n, d, (const float*)mins,
-                                                        (const float*)jumps, sections, (int32_t*)bucket, score);
-      TIP_LAUNCH_CHECK();
-      return TIP_OK;
-    }
-    return launch_kmnc<float, float>(act, n, d, mins, jumps, sections, bucket, bucket_dtype, score, st);
-  }
-  if (act_dtype == TIP_F32 && stat_dtype == TIP_F64)
-    return launch_kmnc<float, double>(act, n, d, mins, jumps, sections, bucket, bucket_dtype, score, st);
-  if (act_dtype == TIP_F64 && stat_dtype == TIP_F32)
-    return launch_kmnc<double, float>(act, n, d, mins, jumps, sections, bucket, bucket_dtype, score, st);
-  if (act_dtype == TIP_F64 && stat_dtype == TIP_F64)
-    return launch_kmnc<double, double>(act, n, d, mins, jumps, sections, bucket, bucket_dtype, score, st);
-  TIP_REQUIRE(false, "dtypes must be TIP_F32 / TIP_F64");
+  if (bucket == nullptr)
+    return kmnc_route<int16_t, false>(act, act_dtype, n, d, mins, jumps, stat_dtype, sections, nullptr, score, st);
+  if (bucket_dtype == TIP_I16)
+    return kmnc_route<int16_t, true>(act, act_dtype, n, d, mins, jumps, stat_dtype, sections, (int16_t*)bucket,
+                                     score, st);
+  return kmnc_route<int32_t, true>(act, act_dtype, n, d, mins, jumps, stat_dtype, sections, (int32_t*)bucket, score,
+                                   st);
+}
+
+extern "C" int tip_kmnc_packed(const void* act, int act_dtype, int64_t n, int64_t d, const void* mins,
+                               const void* jumps, int stat_dtype, int32_t sections, uint32_t* bits, int32_t* score,
+                               void* stream) {
+  TIP_REQUIRE(n >= 0 && d >= 1, "shape");
+  TIP_REQUIRE(sections >= 1, "sections");
+  if (n == 0) return TIP_OK;
+  TIP_REQUIRE(act && mins && jumps && bits && score, "null pointer");
+  return kmnc_route<uint32_t, true>(act, act_dtype, n, d, mins, jumps, stat_dtype, sections, bits, score,
+                                    (cudaStream_t)stream);
 }
 
 extern "C" int64_t tip_pair_pitch(int64_t d, int segments) {

@@ -75,11 +75,14 @@ def device_matrix(layers) -> Optional[torch.Tensor]:
     """Activation traces handed over as device tensors (one [N, ...] tensor or a list of them, the
     form a forward hook produces): the flattened [N, D] matrix on the GPU, else None.  Mirrors
     `_flatten_layers` (surprise.py:62-66) without leaving HBM."""
+    def rows(t):            # explicit width: a -1 cannot be resolved for 0 samples
+        return t.reshape(t.shape[0], int(np.prod(t.shape[1:])))
+
     if isinstance(layers, torch.Tensor):
-        return layers.reshape(layers.shape[0], -1) if layers.is_cuda else None
+        return rows(layers) if layers.is_cuda else None
     if isinstance(layers, (list, tuple)) and len(layers) > 0 and all(isinstance(l, torch.Tensor) and l.is_cuda
                                                                      for l in layers):
-        flat = [l.reshape(l.shape[0], -1) for l in layers]
+        flat = [rows(l) for l in layers]
         return flat[0] if len(flat) == 1 else torch.cat(flat, dim=1)
     return None
 
