@@ -10,7 +10,9 @@ with data_type in {"is_misclassified", "uncertainty_<quantifier>", "<metric>_sco
 metric either a surprise adequacy ("dsa", "pc-lsa", ...) or "<CRITERION>_<param>" ("NAC_0.75", "KMNC_2", ...).
 `load_apfd_values` re-reads such a folder the way src/plotters/eval_apfd_table.py:43-108 does (scores ->
 `np.argsort(-scores)`, CAM orders as stored, APFD against the misclassification mask) — so results written by
-this package are consumable by the reference's table scripts and vice versa.  Host-side I/O only.
+this package are consumable by the reference's table scripts and vice versa.  The active-learning experiment's
+accuracies go to `<out>/active_learning/<case_study>_<model_id>_<metric>_<nominal|ood>.pickle`
+(eval_active_learning.py:134-147, `persist_active_learning`).  Host-side I/O only.
 """
 from __future__ import annotations
 
@@ -65,6 +67,19 @@ def persist_tip(output_folder: str, case_study: str, dataset_id: str, model_id: 
         persist(output_folder, case_study, dataset_id, f"{metric}_cam_order", model_id, np.array(cam_order))
     if times is not None:
         persist_times(output_folder, case_study, dataset_id, model_id, metric, times)
+
+
+def persist_active_learning(output_folder: str, case_study: str, model_id: int, metric: str, ood_or_nom: str,
+                            eval_res: Dict[Tuple[str, str], float]) -> str:
+    """eval_active_learning.py:134-147 (`_save_results_on_file`): one pickle of {(ood_or_nom, observed_or_future):
+    accuracy} per retrained model (metric "original", ood_or_nom "na" for the model before retraining), named as
+    eval_active_learning_table.py:26-59 expects."""
+    folder = os.path.join(output_folder, "active_learning")
+    os.makedirs(folder, exist_ok=True)
+    path = os.path.join(folder, f"{case_study}_{model_id}_{metric}_{ood_or_nom}.pickle")
+    with open(path, "wb") as f:
+        pickle.dump(eval_res, f)
+    return path
 
 
 def approach_name(approach: str, param: str = "", cam: bool = False) -> str:
