@@ -41,8 +41,12 @@ struct tip_comm {
 namespace tip {
 
 constexpr int kHdrBytes = 1024;        // flags[world] at 0, seq at 256, done counter at 260
-constexpr uint64_t kNoneHi64 = 0x7ff0000000000000ull;   // +inf as a double
-constexpr uint64_t kNoneHi32 = 0x7f800000ull;           // +inf as a float
+// "No row of that range on this shard" is a quiet NaN's pattern, above +inf's: a real distance can be +inf
+// (squared differences that overflow), and unsigned order still puts it ahead of "none" (engine.dist_keys).
+constexpr uint64_t kNoneHi64 = 0x7ff8000000000000ull;
+constexpr uint64_t kNoneHi32 = 0x7fc00000ull;
+constexpr uint64_t kInfHi64 = 0x7ff0000000000000ull;
+constexpr uint64_t kInfHi32 = 0x7f800000ull;
 constexpr uint64_t kNoneLo = 0x7fffffffull;
 
 struct CommDev {
@@ -155,11 +159,11 @@ template <typename T>
 __device__ __forceinline__ T bits_dist(uint64_t hi);
 template <>
 __device__ __forceinline__ float bits_dist<float>(uint64_t hi) {
-  return hi >= kNoneHi32 ? __int_as_float(0x7fc00000) : __uint_as_float((uint32_t)hi);
+  return hi > kInfHi32 ? __int_as_float(0x7fc00000) : __uint_as_float((uint32_t)hi);
 }
 template <>
 __device__ __forceinline__ double bits_dist<double>(uint64_t hi) {
-  return hi >= kNoneHi64 ? (double)NAN : __longlong_as_double((long long)hi);
+  return hi > kInfHi64 ? (double)NAN : __longlong_as_double((long long)hi);
 }
 
 __device__ __forceinline__ ulonglong2 reduce_min_records(const CommDev& c, uint32_t seq, int64_t i) {
@@ -203,6 +207,7 @@ __global__ void __launch_bounds__(256) winner_queries_kernel(const CommDev c, co
     dist = gdist[row];
     gid = ggid[row];
   }
+  // only "no row" (the NaN sentinel) or an index outside the training set drops the winner; +inf is a distance
   if (gid < 0 || gid >= n_full || dist != dist) { gid = -1; dist = (T)NAN; }
   if (lane == 0) {
     out_dist[row] = dist;

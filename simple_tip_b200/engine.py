@@ -352,19 +352,45 @@ def count_tile_pairs(q_off: np.ndarray, ranges_per_class, row_tile: int = _lib.R
 # ------------------------------------------------------------------------------------------
 # cross-rank protocol (N_train sharded over the ranks of one NVSwitch box)
 # ------------------------------------------------------------------------------------------
-KEY_NONE_HI32 = 0x7F800000           # +inf as float bits: "this shard has no row of that range"
+# "This shard has no row of that range" is a quiet NaN's bit pattern, which lies above +inf's: a real distance can
+# be +inf (float32 traces whose squared differences overflow), and unsigned / non-negative integer order then still
+# puts every real distance, +inf included, ahead of "none" (csrc/shard.cu uses the same patterns).
+KEY_NONE_HI32 = 0x7FC00000
+KEY_NONE_HI64 = 0x7FF8000000000000
+KEY_INF_HI32 = 0x7F800000
+KEY_INF_HI64 = 0x7FF0000000000000
 KEY_NONE_LO = 0x7FFFFFFF
 P2P_MIN_RECORDS = 1 << 18            # receive slots per rank: 2 x world x 4 MiB
 
 
+def dist_keys(dist: torch.Tensor, none: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Non-negative float32 / float64 distances as int32 / int64 bit patterns that order like the distances, NaN
+    (and rows flagged in `none`) replaced by the "no row" pattern above +inf.  An integer MIN over shards of these
+    keys is the minimum distance, with +inf kept and "none" only where no shard had a row."""
+    f32 = dist.dtype == torch.float32
+    assert f32 or dist.dtype == torch.float64
+    bits = dist.contiguous().view(torch.int32 if f32 else torch.int64)
+    empty = torch.isnan(dist) if none is None else torch.isnan(dist) | none
+    return torch.where(empty, torch.full_like(bits, KEY_NONE_HI32 if f32 else KEY_NONE_HI64), bits)
+
+
+def keys_dist(keys: torch.Tensor) -> torch.Tensor:
+    """Inverse of dist_keys: int32 keys -> float32, int64 -> float64, "no row" (anything above +inf) -> NaN."""
+    f32 = keys.dtype == torch.int32
+    assert f32 or keys.dtype == torch.int64
+    keys = keys.contiguous()
+    dist = keys.view(torch.float32 if f32 else torch.float64)
+    return torch.where(keys > (KEY_INF_HI32 if f32 else KEY_INF_HI64), torch.full_like(dist, float("nan")), dist)
+
+
 def pack_winner_keys(dist: torch.Tensor, gid: torch.Tensor) -> torch.Tensor:
     """float32 distances (>= 0, NaN = no row on this shard) and original indices -> int64 keys
-    (float bits << 32 | index).  Non-negative IEEE floats order like their bit patterns and the
+    (dist_keys << 32 | index).  Non-negative IEEE floats order like their bit patterns and the
     sign bit is clear, so ONE integer MIN all-reduce yields np.min and np.argmin's first occurrence
     (surprise.py:645-647) over all shards.  Plain torch ops: runs on CPU (gloo test) and CUDA."""
     assert dist.dtype == torch.float32
     none = torch.isnan(dist) | (gid < 0)
-    hi = torch.where(none, torch.full_like(dist, float("inf")), dist).view(torch.int32).to(torch.int64)
+    hi = dist_keys(dist, none).to(torch.int64)
     lo = torch.where(none, torch.full_like(gid, KEY_NONE_LO, dtype=torch.int64), gid.to(torch.int64))
     return (hi << 32) | lo
 
@@ -373,9 +399,29 @@ def unpack_winner_keys(keys: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
     """Inverse of pack_winner_keys: (float32 distance with NaN for 'no row anywhere', int64 index or -1)."""
     hi = (keys >> 32).to(torch.int32)
     lo = keys & 0xFFFFFFFF
-    none = (hi >= KEY_NONE_HI32) | (lo >= KEY_NONE_LO)
-    dist = torch.where(none, torch.full((), float("nan"), dtype=torch.float32, device=keys.device), hi.view(torch.float32))
+    none = (hi > KEY_INF_HI32) | (lo >= KEY_NONE_LO)
+    dist = torch.where(none, torch.full((), float("nan"), dtype=torch.float32, device=keys.device), keys_dist(hi))
     return dist, torch.where(none, torch.full_like(lo, -1), lo)
+
+
+WINNER_NONE = torch.iinfo(torch.int64).max
+
+
+def winner_index_candidates(local: torch.Tensor, gkey: torch.Tensor, gid: torch.Tensor) -> torch.Tensor:
+    """Second step of the float64 winner exchange: this rank's original index where its dist_keys `local` hold
+    the global minimum `gkey` (a real row, +inf included), else WINNER_NONE; a MIN over the ranks is then
+    np.argmin's first occurrence."""
+    mine = (local == gkey) & (local <= KEY_INF_HI64) & (gid >= 0)
+    return torch.where(mine, gid.to(torch.int64), torch.full_like(gid, WINNER_NONE, dtype=torch.int64))
+
+
+def winner_from_keys(gkey: torch.Tensor, ggid: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """(global minimum key, reduced winner_index_candidates) -> (float64 distance, int64 index); "none" is
+    decided by the index alone: NaN / -1 where no rank had a row."""
+    none = ggid == WINNER_NONE
+    dist = keys_dist(gkey)
+    return (torch.where(none, torch.full_like(dist, float("nan")), dist),
+            torch.where(none, torch.full_like(ggid, -1), ggid))
 
 
 class P2PExchange:
@@ -508,15 +554,10 @@ class TrainShardComm:
         of the index among the ranks that hold the minimum."""
         if dist_a.dtype == torch.float32:
             return unpack_winner_keys(self.min_(pack_winner_keys(dist_a, gid)))
-        big = torch.iinfo(torch.int64).max
-        local = torch.where(torch.isnan(dist_a), torch.full_like(dist_a, float("inf")), dist_a)
-        gmin = self.min_(local.clone())
-        cand = torch.where((local == gmin) & (gid >= 0), gid.to(torch.int64),
-                           torch.full_like(gid, big, dtype=torch.int64))
-        ggid = self.min_(cand)
-        none = torch.isinf(gmin) | (ggid == big)
-        return (torch.where(none, torch.full_like(gmin, float("nan")), gmin),
-                torch.where(none, torch.full_like(ggid, -1), ggid))
+        local = dist_keys(dist_a, gid < 0)
+        gkey = self.min_(local.clone())
+        ggid = self.min_(winner_index_candidates(local, gkey, gid))
+        return winner_from_keys(gkey, ggid)
 
     def reduce_winners(self, dist_a: torch.Tensor, gid: torch.Tensor, rows: Optional[torch.Tensor] = None,
                        train_full: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
@@ -536,10 +577,8 @@ class TrainShardComm:
         return gmin, ggid, winners
 
     def reduce_min_nan(self, d: torch.Tensor) -> torch.Tensor:
-        """min over ranks where NaN means 'empty range on this shard'."""
-        local = torch.where(torch.isnan(d), torch.full_like(d, float("inf")), d)
-        g = self.min_(local)
-        return torch.where(torch.isinf(g), torch.full_like(g, float("nan")), g)
+        """min over ranks where NaN means 'empty range on this shard' (+inf is a distance like any other)."""
+        return keys_dist(self.min_(dist_keys(d)))
 
     # -- LSA: merge per-shard (max, sum) -------------------------------------------------------
     def reduce_lse(self, mx: torch.Tensor, sm: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
@@ -605,6 +644,10 @@ class NnEngine:
         else:
             self.center = torch.zeros(self.d, dtype=torch.float32, device=self.dev)
             self.t_pack, self.rmax, self.errmax = None, 0.0, 0.0
+        # The filter's window needs finite bounds on the packed train rows.  Rows beyond float32's range (float64
+        # traces above ~3e38, or float32 ones whose squared norm overflows) have none: every query of such an engine
+        # takes the re-rank's exact scan, which has no such limit.
+        self.filter_ok = math.isfinite(self.rmax) and math.isfinite(self.errmax)
         # Stage-2 seeds (short traces / resident-query kernel, where the warm-up of the running minima costs ~15 % of
         # the filter): for every train row an upper bound on the distance to its nearest other-class row = the exact
         # distance to the nearest one inside a fixed stratified sample of the training set, found once at fit time
@@ -730,6 +773,7 @@ class NnEngine:
         speculative: queries whose candidate list is empty or overflowed are only counted in work_buffer(m)[0] (no
         exhaustive-scan launch); the caller checks overflow_count() and repeats the call without it if non-zero."""
         m = q.shape[0] if q_idx is None else q_idx.shape[0]
+        use_filter = use_filter and self.filter_ok
         out_dist = torch.empty(m, dtype=q.dtype, device=self.dev)
         out_pos = torch.empty(m, dtype=torch.int32, device=self.dev)
         out_gid = torch.empty(m, dtype=torch.int32, device=self.dev)
@@ -863,6 +907,7 @@ def dsa_distances(engine: NnEngine, x: torch.Tensor, q_class: torch.Tensor, q_of
     class-sorted queries are rows q_idx[r] of x (the gather is fused into the pack and the re-rank); scatter =
     (idx, n_total, out) — the last re-rank also writes dist_a, dist_b, winner, dist_a / dist_b into out[4, n_total]."""
     sharded = comm is not None and comm.world > 1
+    use_filter = use_filter and engine.filter_ok
     m = x.shape[0] if q_idx is None else q_idx.shape[0]
     if not sharded and engine.table_b is not None and engine.table_b.dtype == x.dtype:
         # fit-time table: stage 1 only, dist_b looked up by the winner's position
@@ -957,6 +1002,7 @@ class DsaPlan:
 
     def __init__(self, engine: "NnEngine", m: int, q_off: np.ndarray, dtype: torch.dtype, use_filter: bool,
                  comm: Optional[TrainShardComm] = None, n_total: Optional[int] = None):
+        use_filter = use_filter and engine.filter_ok
         self.engine = engine
         self.q_off = np.asarray(q_off, dtype=np.int64).copy()
         dev = engine.dev
@@ -1020,49 +1066,46 @@ class DsaPlan:
             # torch.distributed fallback: static exchange buffers written by one graph segment,
             # all-reduced in place (eager), read by the next segment
             f32 = dtype == torch.float32
-            S["keys"] = torch.zeros(self.m, dtype=torch.int64 if f32 else dtype, device=dev)
+            # distances travel as dist_keys (integers, "no row" above +inf), so a real +inf survives the exchange
+            S["keys"] = torch.zeros(self.m, dtype=torch.int64, device=dev)
+            S["local"] = torch.zeros(self.m, dtype=torch.int64, device=dev)
             S["cand"] = torch.zeros(self.m, dtype=torch.int64, device=dev)
-            S["bmin"] = torch.zeros(self.m, dtype=dtype, device=dev)
-            big = torch.iinfo(torch.int64).max
+            S["bmin"] = torch.zeros(self.m, dtype=torch.int32 if f32 else torch.int64, device=dev)
 
             def seg_a():
                 gather()
                 la, _, lg, _ = engine.search(self.x, self.q_class, self.q_off, _lib.RANGE_SAME_CLASS, use_filter)
-                S["la"], S["lg"] = la, lg
+                S["lg"] = lg
                 if f32:
                     S["keys"].copy_(pack_winner_keys(la, lg))
                 else:
-                    S["keys"].copy_(torch.where(torch.isnan(la), torch.full_like(la, float("inf")), la))
+                    S["local"].copy_(dist_keys(la, lg < 0))
+                    S["keys"].copy_(S["local"])
 
             def exch_1():
                 self.comm.min_(S["keys"])
                 if not f32:
-                    la = torch.where(torch.isnan(S["la"]), torch.full_like(S["la"], float("inf")), S["la"])
-                    S["cand"].copy_(torch.where((la == S["keys"]) & (S["lg"] >= 0), S["lg"].to(torch.int64),
-                                                torch.full_like(S["cand"], big)))
+                    S["cand"].copy_(winner_index_candidates(S["local"], S["keys"], S["lg"]))
                     self.comm.min_(S["cand"])
 
             def seg_b():
                 if f32:
                     gmin, ggid = unpack_winner_keys(S["keys"])
                 else:
-                    none = torch.isinf(S["keys"]) | (S["cand"] == big)
-                    gmin = torch.where(none, torch.full_like(S["keys"], float("nan")), S["keys"])
-                    ggid = torch.where(none, torch.full_like(S["cand"], -1), S["cand"])
+                    gmin, ggid = winner_from_keys(S["keys"], S["cand"])
                 state2 = engine.query_state(self.m)
                 a, gid, winners = winner_queries(engine, None, gmin.contiguous(), ggid.to(torch.int32).contiguous(),
                                                  self.m, dtype, state2)
                 S["a"], S["gid"] = a, gid
                 pre = state2 if (use_filter and engine.has_items(self.q_off, _lib.RANGE_OTHER_CLASSES)) else None
                 lb = engine.search(winners, self.q_class, self.q_off, _lib.RANGE_OTHER_CLASSES, use_filter, prepacked=pre)[0]
-                S["bmin"].copy_(torch.where(torch.isnan(lb), torch.full_like(lb, float("inf")), lb))
+                S["bmin"].copy_(dist_keys(lb))
 
             def exch_2():
                 self.comm.min_(S["bmin"])
 
             def seg_c():
-                b = torch.where(torch.isinf(S["bmin"]), torch.full_like(S["bmin"], float("nan")), S["bmin"])
-                scatter(S["a"], b, S["gid"])
+                scatter(S["a"], keys_dist(S["bmin"]), S["gid"])
 
             segments = [(seg_a, True), (exch_1, False), (seg_b, True), (exch_2, False), (seg_c, True)]
 

@@ -279,6 +279,24 @@ def _worker(rank, world, port, q):
         # a class missing on one shard / everywhere
         nan_case = comm.reduce_min_nan(torch.tensor([float("nan"), 1.0 + rank]))
         assert np.isnan(nan_case[0].item()) and nan_case[1].item() == 1.0
+        # a real +inf distance (squared differences that overflow) is a row, not "no row": it survives the exchange
+        inf, nan = float("inf"), float("nan")
+        for dt in (torch.float32, torch.float64):
+            own = [inf, inf, nan, inf, nan] if rank == 0 else [nan, inf, nan, 5.0, -nan]
+            g = comm.reduce_min_nan(torch.tensor(own, dtype=dt))
+            assert g.dtype == dt and list(g[[0, 1, 3]].tolist()) == [inf, inf, 5.0] and np.isnan(g[[2, 4]].numpy()).all()
+            i_d, i_g = comm.reduce_winner_index(torch.tensor([inf, inf, nan, inf], dtype=dt),
+                                                torch.tensor([4 + rank, 9 - rank, -1, -1 if rank else 3]))
+            assert i_d.dtype == dt and i_d[[0, 1, 3]].tolist() == [inf, inf, inf] and np.isnan(i_d[2].item())
+            assert i_g.tolist() == [4, 8, -1, 3]
+        # stage 1 -> stage 2 with every training row far out: the winners' traces are gathered, dist_b = inf
+        big = np.full((4, 3), 3e19, dtype=np.float32)
+        big[1] = 0.0
+        w_da, w_gid, w_rows = comm.reduce_winners(torch.tensor([inf, 0.0] if rank == 0 else [inf, nan]),
+                                                  torch.tensor([2 + rank, 1] if rank == 0 else [2 + rank, -1]),
+                                                  None, torch.from_numpy(big))
+        assert w_da.tolist() == [inf, 0.0] and w_gid.tolist() == [2, 1]
+        assert np.array_equal(w_rows.numpy(), big[[2, 1]])
         q.put((rank, "ok"))
     except Exception as e:  # pragma: no cover
         import traceback
@@ -362,6 +380,7 @@ def test_winner_keys_order_like_numpy_argmin():
     d[::7] = d[0]                                 # exact ties
     d[5] = 0.0
     d[9] = np.float32(1e-45)                      # subnormal
+    d[100:4096:301] = np.inf                      # a real distance whose squares overflowed, tied among themselves
     gid = rng.permutation(4096).astype(np.int64)
     keys = E.pack_winner_keys(torch.from_numpy(d), torch.from_numpy(gid))
     assert (keys >= 0).all()
@@ -369,10 +388,19 @@ def test_winner_keys_order_like_numpy_argmin():
     assert np.array_equal(np.argsort(keys.numpy(), kind="stable"), order)
     back_d, back_g = E.unpack_winner_keys(keys)
     assert np.array_equal(back_d.numpy(), d) and np.array_equal(back_g.numpy(), gid)
-    none = E.pack_winner_keys(torch.tensor([float("nan"), 1.0]), torch.tensor([3, -1]))
+    none = E.pack_winner_keys(torch.tensor([float("nan"), 1.0, -float("nan"), float("inf")]), torch.tensor([3, -1, 4, -1]))
     assert (none > keys.max()).all()
     nd, ng = E.unpack_winner_keys(none)
     assert np.isnan(nd.numpy()).all() and (ng.numpy() == -1).all()
+    # the distance-only keys of the other exchanges: same order, +inf below "none", both dtypes
+    for dt in (torch.float32, torch.float64):
+        v = torch.tensor([0.0, 1e-300 if dt == torch.float64 else 1e-45, 2.0, float("inf"), float("nan"), -float("nan")],
+                         dtype=dt)
+        k = E.dist_keys(v)
+        assert k.dtype == (torch.int32 if dt == torch.float32 else torch.int64)
+        assert (k[:3] < k[3]).all() and (k[3] < k[4]).all() and k[4] == k[5]
+        back = E.keys_dist(k)
+        assert back.dtype == dt and back[:4].tolist() == v[:4].tolist() and torch.isnan(back[4:]).all()
 
 
 def test_bench_clock_sampler_reports_rows_of_the_timed_region():
