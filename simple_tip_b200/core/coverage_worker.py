@@ -28,7 +28,8 @@ class CoverageWorker(HookedModelHandler):
     in badges of `batch_size` on the model's device.  Every timer ends with a synchronise of the current CUDA device
     (and the model's, when that is another one), so device work is inside the phase that launched it.
 
-    Writing the reference's result files (eval_prioritization.py:174-193):
+    Writing the reference's result files (eval_prioritization.py:174-193; `prioritization.evaluate` runs the whole
+    experiment, this arm included):
 
         worker = CoverageWorker(model, [1, 2, 4, 5], x_train)
         for ds_name, x in {"nominal": x_test, "ood": x_ood}.items():

@@ -33,7 +33,8 @@ class SurpriseHandler(HookedModelHandler):
     NumPy arrays in the SA's dtype.  Every timer ends with a synchronise of the current CUDA device (and the model's,
     when that is another one), so device work is inside the phase that launched it.
 
-    Writing the reference's result files (eval_prioritization.py:174-193):
+    Writing the reference's result files (eval_prioritization.py:114-154; `prioritization.evaluate` runs the whole
+    experiment, this arm included):
 
         res = SurpriseHandler(model, [3], x_train).evaluate_all({"nominal": x_test, "ood": x_ood})
         for sa_name, per_ds in res.items():
