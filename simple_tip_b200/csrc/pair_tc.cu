@@ -19,9 +19,13 @@
 // the per-row reductions finish with two quad shuffles.  The consumer warpgroups drift out of phase, so one's MMAs
 // overlap another's reduction.  The resident MODE_NN kernel has three consumer warpgroups on 192-row query tiles
 // (512 threads; warpgroup 0 hands registers to the consumers with setmaxnreg): while one reduces, the other two
-// keep the tensor core busy, and each train tile fetched from L2 feeds 1.5x the MMAs.  A consumer warpgroup whose
-// rows all lie past the item's query rows issues no MMAs.  Every other instantiation has two consumer warpgroups on
-// 128-row tiles (384 threads).
+// keep the tensor core busy, and each train tile fetched from L2 feeds 1.5x the MMAs.  Handing the tensor core from
+// one warpgroup to the next (each issues a tile's MMAs only after the previous one has issued its own) was measured
+// slower: alone, one warpgroup's nine m64n128k16 run at about half the tensor core's rate, so the three warpgroups'
+// MMAs take longer one after another than together (DESIGN.md §8).  At d = 128 its consumers hold most of the query
+// tile's K steps in registers (wgmma with a register A operand), so their MMAs read mostly the train tile from shared
+// memory.  A consumer warpgroup whose rows all lie past the item's query rows issues no MMAs.  Every other
+// instantiation has two consumer warpgroups on 128-row tiles (384 threads).
 // Pipeline: kStages-deep shared-memory ring (full/empty mbarriers, TMA -> wgmma).  Streaming variant:
 // one commit group per K chunk, each waited for and its stage released before the next chunk.
 // Resident-query variant (RESA, short packed rows): the query tile's K chunks are loaded once per run
@@ -205,6 +209,15 @@ __device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t adesc,
         : TIP_ACC8(0), TIP_ACC8(8), TIP_ACC8(16), TIP_ACC8(24), TIP_ACC8(32), TIP_ACC8(40), TIP_ACC8(48), TIP_ACC8(56)
         : "l"(adesc), "l"(bdesc), "r"(accumulate));
   }
+}
+// The same with A from registers: the m64 x k16 bf16 fragment of this thread in the layout ldmatrix.x4 gives
+__device__ __forceinline__ void wgmma_m64n128k16_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t bdesc,
+                                                    uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 " TIP_WGMMA_REGS ", {%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}"
+      : TIP_ACC8(0), TIP_ACC8(8), TIP_ACC8(16), TIP_ACC8(24), TIP_ACC8(32), TIP_ACC8(40), TIP_ACC8(48), TIP_ACC8(56)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
 }
 #undef TIP_ACC8
 #undef TIP_WGMMA_REGS
@@ -563,6 +576,14 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     uint32_t phase = 0, a_phase = 0;
     int a_row0 = -1;
     bool first_item = true;
+    // Resident MODE_NN with 9 K16 steps (d = 128): each warp loads its rows of the query tile into registers once per
+    // query tile, so most MMAs read only the train tile from shared memory.  With both operands there, an m64n128k16
+    // reads 6 KB, and three warpgroups at the tensor rate would read ~94 of shared memory's 128 bytes per clock.  Only
+    // the first kRegK steps fit in the consumers' 152 registers without spills; the last two come from shared memory.
+    constexpr bool kRegA = MODE == MODE_NN && RESA && !F16;
+    const bool reg_a = kRegA && k16 == kRsMaxK16;
+    constexpr int kRegK = 7;
+    uint32_t afr[kRegK][4];
     int tl_tile0 = 0;           // timeline index of the item's first tile
     int qt = 0;                 // MODE_NN: tiles handed to the drain so far (mailbox qt & 1)
     for (int k = 0;; k++) {
@@ -628,6 +649,18 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
           if (lane == 0) mbar_arrive(a_empty);
         }
         mbar_wait<!kSplitRegs>(a_full, a_phase);
+        if (reg_a) {
+          // ldmatrix.x4: lane l addresses row l % 16 of the warp's 16 rows, 8 K elements (16 bytes) at (l / 16) * 8;
+          // 16-byte unit j of a 128-byte row r sits at unit j ^ (r % 8) (SWIZZLE_128B)
+          const int r = g * 64 + (cw & 3) * 16 + (lane & 15);
+#pragma unroll
+          for (int s = 0; s < kRegK; s++) {
+            const int j = (s & 3) * 2 + (lane >> 4);
+            const uint32_t addr = base + (uint32_t)(s >> 2) * L::kABytes + (uint32_t)r * 128 + (uint32_t)((j ^ (r & 7)) << 4);
+            asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+                         : "=r"(afr[s][0]), "=r"(afr[s][1]), "=r"(afr[s][2]), "=r"(afr[s][3]) : "r"(addr) : "memory");
+          }
+        }
         a_phase ^= 1u;
         a_row0 = it.q_row0;
       }
@@ -651,16 +684,34 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
           }
           return;
         }
-        for (int c = 0; c < nchunks; c++) {
-          mbar_wait<!kSplitRegs>(full_bar(stage), phase);
-          const uint32_t a_addr = base + (uint32_t)c * L::kABytes + (uint32_t)g * 64 * 128;
-          const uint32_t b_addr = b_ring + (uint32_t)stage * kBBytes;
-          const uint64_t adesc = smem_desc(a_addr), bdesc = smem_desc(b_addr);
-          const int nm = min(4, k16 - 4 * c);
-          wgmma_fence();
-          wgmma_m64n128k16<F16>(a, adesc, bdesc, c > 0 ? 1u : 0u);
-          for (int kk = 1; kk < nm; kk++) wgmma_m64n128k16<F16>(a, adesc + 2u * kk, bdesc + 2u * kk, 1u);
-          if (++stage == kStages) { stage = 0; phase ^= 1u; }
+        if (kRegA && reg_a) {
+#pragma unroll
+          for (int c = 0; c < (kRsMaxK16 + 3) / 4; c++) {
+            mbar_wait<!kSplitRegs>(full_bar(stage), phase);
+            const uint64_t bdesc = smem_desc(b_ring + (uint32_t)stage * kBBytes);
+            wgmma_fence();
+#pragma unroll
+            for (int kk = 0; kk < 4 && 4 * c + kk < kRsMaxK16; kk++) {
+              if (4 * c + kk < kRegK)
+                wgmma_m64n128k16_rs(a, afr[4 * c + kk], bdesc + 2u * kk, (c | kk) ? 1u : 0u);
+              else
+                wgmma_m64n128k16<F16>(a, smem_desc(base + (uint32_t)c * L::kABytes + (uint32_t)g * 64 * 128) + 2u * kk,
+                                      bdesc + 2u * kk, 1u);
+            }
+            if (++stage == kStages) { stage = 0; phase ^= 1u; }
+          }
+        } else {
+          for (int c = 0; c < nchunks; c++) {
+            mbar_wait<!kSplitRegs>(full_bar(stage), phase);
+            const uint32_t a_addr = base + (uint32_t)c * L::kABytes + (uint32_t)g * 64 * 128;
+            const uint32_t b_addr = b_ring + (uint32_t)stage * kBBytes;
+            const uint64_t adesc = smem_desc(a_addr), bdesc = smem_desc(b_addr);
+            const int nm = min(4, k16 - 4 * c);
+            wgmma_fence();
+            wgmma_m64n128k16<F16>(a, adesc, bdesc, c > 0 ? 1u : 0u);
+            for (int kk = 1; kk < nm; kk++) wgmma_m64n128k16<F16>(a, adesc + 2u * kk, bdesc + 2u * kk, 1u);
+            if (++stage == kStages) { stage = 0; phase ^= 1u; }
+          }
         }
         wgmma_commit();
         acc_fence(a);
