@@ -48,6 +48,8 @@
  *   tip_col_var         src/core/surprise.py:421,433 LSA's column selection: np.var(x, axis=0), bit for bit
  *   tip_whiten_dmma     scipy==1.4.1 gaussian_kernel_estimate: dataset . cholesky(inv_cov) for the training rows
  *                       of LSA's device fit, fp64 DMMA (the covariance reuses tip_gmm_scatter)
+ *   tip_levenshtein     src/core/text_corruptor.py:282-309 TextCorruptor._calculate_distances: the all-pairs
+ *                       polyleven.levenshtein matrix of the dictionary, bit-parallel (Myers / Hyyro)
  */
 #ifndef B200TIP_H
 #define B200TIP_H
@@ -558,6 +560,17 @@ int tip_col_var(const void* x, int dtype, int64_t n, int64_t d, void* var, doubl
                 void* stream);
 int tip_whiten_dmma(const void* x, int dtype, int64_t m, int64_t d_in, const int32_t* cols, int64_t d_out,
                     const double* mu, const double* w_lower, float* out, void* stream);
+
+/* ---- IMDB-C's dictionary distances (TextCorruptor) -------------------------------------------------------
+ * tip_levenshtein: out[na x nb] (uint8, row-major, int64 indexing) = unit-cost Levenshtein distance (insert, delete,
+ * substitute) of word a_i and word b_j, as polyleven.levenshtein computes it on Python str.  A word is a run of int32
+ * code-point ids (equal ids = equal code points): a_ids[a_off[i] .. a_off[i+1]), a_off has na + 1 entries, likewise
+ * b.  Ids below 64 get a shared-memory match mask, so the caller numbers the most frequent code points first; any
+ * id >= 0 is exact.  max_len >= the longest word of a and b, <= 255 (so every distance fits in a byte).
+ * symmetric != 0: a and b are the same block (same pointers, na == nb); each unordered pair is computed once and
+ * written to both halves.  na == 0 or nb == 0 launches nothing. */
+int tip_levenshtein(const int32_t* a_ids, const int32_t* a_off, int64_t na, const int32_t* b_ids,
+                    const int32_t* b_off, int64_t nb, int32_t max_len, int symmetric, uint8_t* out, void* stream);
 
 /* ---- bring-up / validation: plain accumulator dump ------------------------------------
  * out[256*256] (fp32, row-major, leading dimension 256) = tail-augmented dot products of q rows

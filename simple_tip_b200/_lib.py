@@ -109,6 +109,7 @@ _SIGNATURES = {
     "tip_cov_location": (C.c_int, [_vp, C.c_int, _i64, _i64, _vp, _vp, _vp, _vp]),
     "tip_col_var": (C.c_int, [_vp, C.c_int, _i64, _i64, _vp, _vp, _vp, _vp]),
     "tip_whiten_dmma": (C.c_int, [_vp, C.c_int, _i64, _i64, _vp, _i64, _vp, _vp, _vp, _vp]),
+    "tip_levenshtein": (C.c_int, [_vp, _vp, _i64, _vp, _vp, _i64, _i32, C.c_int, _vp, _vp]),
 }
 
 _lock = threading.Lock()

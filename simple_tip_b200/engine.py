@@ -1840,3 +1840,64 @@ def silhouette_samples(x: torch.Tensor, labels: torch.Tensor, n_clusters: int,
     _lib.check(lib.tip_sil_finish(_p(part), n, slots, _p(slot_dev), _p(lab_sorted), _p(counts32), _p(order32), _p(out),
                                   _stream()), "tip_sil_finish")
     return out
+
+
+LEV_MAX_LEN = 255         # distances are stored as uint8
+
+
+def check_word_lengths(words: Sequence[str]) -> np.ndarray:
+    """int64 code-point lengths of words; ValueError naming the first word longer than LEV_MAX_LEN."""
+    lengths = np.fromiter(map(len, words), dtype=np.int64, count=len(words))
+    too_long = np.flatnonzero(lengths > LEV_MAX_LEN)
+    if too_long.size:
+        k = int(too_long[0])
+        raise ValueError(f"word {k} has {int(lengths[k])} code points; Levenshtein distances are stored as uint8, "
+                         f"so words are limited to {LEV_MAX_LEN}")
+    return lengths
+
+
+def encode_words(words: Sequence[str]) -> Tuple[np.ndarray, np.ndarray]:
+    """(ids int32, offsets int32 [len(words) + 1]) of a word list for tip_levenshtein: one id per Unicode code point
+    (as Python's len counts them), numbered by descending frequency (ties by code point), so that the most common
+    ones get the kernel's shared-memory match masks.  Raises ValueError, naming the first such word, when a word is
+    longer than LEV_MAX_LEN code points: its distances would not fit the uint8 matrix."""
+    lengths = check_word_lengths(words)
+    offsets = np.zeros(len(words) + 1, dtype=np.int64)
+    np.cumsum(lengths, out=offsets[1:])
+    if offsets[-1] >= 2 ** 31:
+        raise ValueError("the words have 2^31 code points or more; tip_levenshtein indexes them with int32")
+    cps = np.frombuffer("".join(words).encode("utf-32-le", "surrogatepass"), dtype="<u4")
+    uniq, inverse, counts = np.unique(cps, return_inverse=True, return_counts=True)
+    rank = np.empty(uniq.shape[0], dtype=np.int32)
+    rank[np.lexsort((uniq, -counts))] = np.arange(uniq.shape[0], dtype=np.int32)
+    return rank[inverse.reshape(-1)], offsets.astype(np.int32)
+
+
+def levenshtein(a_words: Sequence[str], b_words: Optional[Sequence[str]] = None) -> torch.Tensor:
+    """uint8 [A, B] device matrix of unit-cost Levenshtein distances (polyleven.levenshtein on str) between every
+    word of a_words and every word of b_words (tip_levenshtein).  b_words None: the square matrix of a_words, each
+    unordered pair computed once and mirrored.  Words longer than LEV_MAX_LEN code points raise ValueError before
+    anything reaches the device."""
+    if b_words is not None:
+        check_word_lengths(b_words)          # names the word by its index in b_words
+    words = list(a_words) + ([] if b_words is None else list(b_words))
+    ids, offsets = encode_words(words)
+    dev = require_cuda()
+    na = len(a_words)
+    nb = na if b_words is None else len(words) - na
+    out = torch.empty((na, nb), dtype=torch.uint8, device=dev)
+    if na == 0 or nb == 0:
+        return out
+    lib = _lib.load()
+    max_len = int(np.max(np.diff(offsets)))
+    ids_d = torch.from_numpy(np.concatenate([ids, np.zeros(1, np.int32)])).to(dev)   # never empty
+    off_d = torch.from_numpy(offsets).to(dev)
+    if b_words is None:
+        a_ids = b_ids = ids_d
+        a_off = b_off = off_d
+    else:
+        a_ids, a_off = ids_d, off_d[:na + 1]
+        b_ids, b_off = ids_d[int(offsets[na]):], off_d[na:] - int(offsets[na])
+    _lib.check(lib.tip_levenshtein(_p(a_ids), _p(a_off), na, _p(b_ids), _p(b_off), nb, max_len,
+                                   int(b_words is None), _p(out), _stream()), "tip_levenshtein")
+    return out

@@ -1,7 +1,6 @@
 """Drop-in overlay of the reference's `src.core` package (H100 / sm_90a implementations).
 
-Modules this overlay does not provide (e.g. `src.core.text_corruptor`, used by
-src/dnn_test_prio/case_study_imdb.py:12) fall through to the reference's own `src/core` when it
+Modules this overlay does not provide fall through to the reference's own `src/core` when it
 is on sys.path after this repository: the package path is extended over every `src/core`
 directory of the `src` namespace package.
 """
