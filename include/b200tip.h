@@ -50,6 +50,11 @@
  *                       of LSA's device fit, fp64 DMMA (the covariance reuses tip_gmm_scatter)
  *   tip_levenshtein     src/core/text_corruptor.py:282-309 TextCorruptor._calculate_distances: the all-pairs
  *                       polyleven.levenshtein matrix of the dictionary, bit-parallel (Myers / Hyyro)
+ *   tip_tok_count       case_study_imdb.py:321-336 keras_preprocessing 1.1.2 text_to_word_sequence: words per text
+ *   tip_tok_emit        ... each word's bytes (offset, length, text, hash) in Keras' iteration order
+ *   tip_tok_vocab_table ... the vocabulary's hash table
+ *   tip_tok_fit         Tokenizer.fit_on_texts: word_counts, first occurrences and word_docs
+ *   tip_tok_lookup      Tokenizer.texts_to_sequences and pad_sequences, fused
  */
 #ifndef B200TIP_H
 #define B200TIP_H
@@ -571,6 +576,47 @@ int tip_whiten_dmma(const void* x, int dtype, int64_t m, int64_t d_in, const int
  * written to both halves.  na == 0 or nb == 0 launches nothing. */
 int tip_levenshtein(const int32_t* a_ids, const int32_t* a_off, int64_t na, const int32_t* b_ids,
                     const int32_t* b_off, int64_t nb, int32_t max_len, int symmetric, uint8_t* out, void* stream);
+
+/* ---- the IMDB case study's inputs: Keras' word tokenizer (keras_preprocessing 1.1.2) -------------------------
+ * Texts are one UTF-8 byte buffer text[text_off[t] .. text_off[t+1]) per text (n_texts + 1 offsets).  A word is a
+ * maximal run of bytes that are not separators; separators are ASCII bytes, bit b of (sep_hi:sep_lo) set = byte b
+ * separates (the filters and the split character).  Words are numbered text-major, position-minor.
+ * tip_tok_count: lower != 0 lowercases ASCII A-Z in place; word_off[n_texts + 1] = exclusive scan of the words per
+ * text (word_off[n_texts] = the total).
+ * tip_tok_emit: w_start (byte offset), w_len, w_text and w_hash (64-bit hash of the bytes, low hash_bits bits
+ * kept, 1..64; 64 in normal use, fewer only to force collisions) of every word; word_off from tip_tok_count.
+ * tip_tok_vocab_table: the vocabulary (distinct words arena[v_start[i] .. + v_len[i])) into an open-addressing
+ * table keys[cap] (cap a power of two >= 2 nv, <= 2^31; key = entry i, empty = ~0); v_hash[nv] out; first
+ * (nullable) [cap] = the key of each slot, ~0 when empty (the fit's first-occurrence array).
+ * tip_tok_fit: adds the n_words words to a table built by tip_tok_vocab_table with cap >= 2 (nv + n_words) and
+ * first != nullptr.  A new word claims a slot with key nv + its first ordinal; words are compared by hash, length
+ * and bytes, so collisions never merge words.  count / docs [cap] scratch, doc_keys [doc_cap] scratch (power of
+ * two >= 2 n_words).  out [5][out_cap] (out_cap >= nv + n_words), one column per word this call saw, in no order:
+ * first-occurrence key, occurrences, texts containing it, and for a new word (key >= nv) its first occurrence's
+ * byte offset and length (else -1, 0); *n_out = the number of columns.
+ * tip_tok_lookup: every word's id = v_index[its vocabulary entry] (keys from tip_tok_vocab_table), dropped when
+ * unknown or when num_words != 0 and id >= num_words.  w_id [n_words] scratch; kept_off [n_texts + 1] = exclusive
+ * scan of the kept ids per text; ragged (nullable, >= n_words entries) = the kept ids at kept_off; padded
+ * (nullable) [n_texts][maxlen] = pad_sequences of the kept ids (maxlen >= 1, padding / truncating "pre" when
+ * pre_padding / pre_truncating != 0, else "post", fill value).  n_texts == 0 launches nothing. */
+int tip_tok_count(uint8_t* text, const int64_t* text_off, int64_t n_texts, uint64_t sep_lo, uint64_t sep_hi, int lower,
+                  int64_t* word_off, void* stream);
+int tip_tok_emit(const uint8_t* text, const int64_t* text_off, int64_t n_texts, uint64_t sep_lo, uint64_t sep_hi,
+                 const int64_t* word_off, int64_t n_words, int32_t hash_bits, int64_t* w_start, int32_t* w_len,
+                 int32_t* w_text, uint64_t* w_hash, void* stream);
+int tip_tok_vocab_table(const uint8_t* arena, const int64_t* v_start, const int32_t* v_len, int64_t nv,
+                        int32_t hash_bits, uint64_t* v_hash, uint64_t* keys, uint64_t* first, int64_t cap, void* stream);
+int tip_tok_fit(const uint8_t* text, const int64_t* w_start, const int32_t* w_len, const int32_t* w_text,
+                const uint64_t* w_hash, int64_t n_words, const uint8_t* arena, const int64_t* v_start,
+                const int32_t* v_len, const uint64_t* v_hash, int64_t nv, uint64_t* keys, uint64_t* first,
+                uint64_t* count, uint64_t* docs, int64_t cap, uint64_t* doc_keys, int64_t doc_cap, int64_t* out,
+                int64_t out_cap, uint64_t* n_out, void* stream);
+int tip_tok_lookup(const uint8_t* text, const int64_t* w_start, const int32_t* w_len, const uint64_t* w_hash,
+                   int64_t n_words, const uint8_t* arena, const int64_t* v_start, const int32_t* v_len,
+                   const uint64_t* v_hash, const int32_t* v_index, int64_t nv, const uint64_t* keys, int64_t cap,
+                   int64_t num_words, const int64_t* word_off, int64_t n_texts, int32_t* w_id, int64_t* kept_off,
+                   int32_t* ragged, int32_t* padded, int64_t maxlen, int pre_padding, int pre_truncating,
+                   int32_t value, void* stream);
 
 /* ---- bring-up / validation: plain accumulator dump ------------------------------------
  * out[256*256] (fp32, row-major, leading dimension 256) = tail-augmented dot products of q rows

@@ -36,7 +36,7 @@ class WorkItem(C.Structure):
                 ("slot", C.c_int32), ("reserved", C.c_int32)]
 
 
-_vp, _i32, _i64, _f32 = C.c_void_p, C.c_int32, C.c_int64, C.c_float
+_vp, _i32, _i64, _u64, _f32 = C.c_void_p, C.c_int32, C.c_int64, C.c_uint64, C.c_float
 
 # name -> (restype, argtypes); mirrors include/b200tip.h one to one
 _SIGNATURES = {
@@ -110,6 +110,13 @@ _SIGNATURES = {
     "tip_col_var": (C.c_int, [_vp, C.c_int, _i64, _i64, _vp, _vp, _vp, _vp]),
     "tip_whiten_dmma": (C.c_int, [_vp, C.c_int, _i64, _i64, _vp, _i64, _vp, _vp, _vp, _vp]),
     "tip_levenshtein": (C.c_int, [_vp, _vp, _i64, _vp, _vp, _i64, _i32, C.c_int, _vp, _vp]),
+    "tip_tok_count": (C.c_int, [_vp, _vp, _i64, _u64, _u64, C.c_int, _vp, _vp]),
+    "tip_tok_emit": (C.c_int, [_vp, _vp, _i64, _u64, _u64, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp]),
+    "tip_tok_vocab_table": (C.c_int, [_vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _i64, _vp]),
+    "tip_tok_fit": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _i64, _vp,
+                              _i64, _vp, _i64, _vp, _vp]),
+    "tip_tok_lookup": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _i64, _i64, _vp, _i64,
+                                 _vp, _vp, _vp, _vp, _i64, C.c_int, C.c_int, _i32, _vp]),
 }
 
 _lock = threading.Lock()

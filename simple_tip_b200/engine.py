@@ -1901,3 +1901,127 @@ def levenshtein(a_words: Sequence[str], b_words: Optional[Sequence[str]] = None)
     _lib.check(lib.tip_levenshtein(_p(a_ids), _p(a_off), na, _p(b_ids), _p(b_off), nb, max_len,
                                    int(b_words is None), _p(out), _stream()), "tip_levenshtein")
     return out
+
+
+# ---- Keras' word tokenizer (tokenizer.cu) ------------------------------------------------------------------------
+TOK_HASH_BITS = 64        # hash width of the word tables; narrower only to force collisions in tests
+
+
+def _pow2_at_least(n: int) -> int:
+    return 1 << max(1, int(n - 1).bit_length())
+
+
+def separator_mask(chars: str) -> Tuple[int, int]:
+    """(low, high) 64-bit halves of the 128-bit mask of separator bytes; every char must be ASCII."""
+    mask = 0
+    for ch in chars:
+        if ord(ch) >= 128:
+            raise ValueError(f"separator {ch!r} is not ASCII")
+        mask |= 1 << ord(ch)
+    return mask & (2 ** 64 - 1), mask >> 64
+
+
+def encode_texts(texts: Sequence[str], lower: bool) -> Tuple[bytes, np.ndarray]:
+    """UTF-8 bytes ("surrogatepass": equal str <-> equal bytes) of the texts and their int64 offsets [n + 1].  With
+    lower, texts that are not ASCII are lowered here by str.lower(); the device lowers ASCII A-Z, which is
+    str.lower() for ASCII text and changes nothing after it."""
+    enc = [(t.lower() if lower and not t.isascii() else t).encode("utf-8", "surrogatepass") for t in texts]
+    off = np.zeros(len(enc) + 1, dtype=np.int64)
+    np.cumsum(np.fromiter(map(len, enc), dtype=np.int64, count=len(enc)), out=off[1:])
+    if len(enc) and int(np.max(np.diff(off))) >= 2 ** 31:
+        raise ValueError("a text has 2^31 bytes or more; word lengths are int32")
+    return b"".join(enc), off
+
+
+class TokWords:
+    """The words of one batch of texts on the device (tip_tok_count + tip_tok_emit): the texts' bytes (ASCII
+    lowered), word_off [n_texts + 1], and per word (text-major, position-minor) start, length, text and hash."""
+
+    def __init__(self, raw: bytes, off: np.ndarray, sep: Tuple[int, int], lower: bool, hash_bits: int):
+        dev = require_cuda()
+        lib = _lib.load()
+        self.n_texts = len(off) - 1
+        self.text = torch.from_numpy(np.frombuffer(bytearray(raw) + b"\0", dtype=np.uint8)).to(dev)   # never empty
+        self.text_off = torch.from_numpy(off).to(dev)
+        self.word_off = torch.empty(self.n_texts + 1, dtype=torch.int64, device=dev)
+        _lib.check(lib.tip_tok_count(_p(self.text), _p(self.text_off), self.n_texts, sep[0], sep[1], int(lower),
+                                     _p(self.word_off), _stream()), "tip_tok_count")
+        self.n_words = int(self.word_off[-1].item())
+        n = max(self.n_words, 1)
+        self.start = torch.empty(n, dtype=torch.int64, device=dev)
+        self.length = torch.empty(n, dtype=torch.int32, device=dev)
+        self.text_id = torch.empty(n, dtype=torch.int32, device=dev)
+        self.hash = torch.empty(n, dtype=torch.int64, device=dev)
+        _lib.check(lib.tip_tok_emit(_p(self.text), _p(self.text_off), self.n_texts, sep[0], sep[1], _p(self.word_off),
+                                    self.n_words, hash_bits, _p(self.start), _p(self.length), _p(self.text_id),
+                                    _p(self.hash), _stream()), "tip_tok_emit")
+
+
+class TokVocab:
+    """A tokenizer's vocabulary on the device: its words' bytes (arena, start, length, in word_counts order), their
+    Keras indexes, and (built on first use) the open-addressing table that tip_tok_lookup probes."""
+
+    def __init__(self, arena: bytes, start: np.ndarray, length: np.ndarray, index: np.ndarray, hash_bits: int):
+        dev = require_cuda()
+        self.n = len(start)
+        self.hash_bits = hash_bits
+        self.arena = torch.from_numpy(np.frombuffer(bytearray(arena) + b"\0", dtype=np.uint8)).to(dev)
+        self.start = torch.from_numpy(np.concatenate([start.astype(np.int64), [0]])).to(dev)
+        self.length = torch.from_numpy(np.concatenate([length.astype(np.int32), [0]]).astype(np.int32)).to(dev)
+        self.index = torch.from_numpy(np.concatenate([index, [0]]).astype(np.int32)).to(dev)
+        self.hash = torch.empty(self.n + 1, dtype=torch.int64, device=dev)
+        self.keys, self.cap = None, 0
+
+    def table(self, cap: int, first: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """keys [cap] of a fresh table holding the vocabulary (tip_tok_vocab_table); first, when given, gets each
+        slot's key (the fit's first-occurrence array)."""
+        keys = torch.empty(cap, dtype=torch.int64, device=self.hash.device)
+        _lib.check(_lib.load().tip_tok_vocab_table(_p(self.arena), _p(self.start), _p(self.length), self.n,
+                                                   self.hash_bits, _p(self.hash), _p(keys), _p(first), cap, _stream()),
+                   "tip_tok_vocab_table")
+        return keys
+
+    def lookup_table(self) -> Tuple[Optional[torch.Tensor], int]:
+        if self.keys is None and self.n:
+            self.cap = _pow2_at_least(2 * self.n)
+            self.keys = self.table(self.cap)
+        return self.keys, self.cap
+
+
+def tok_fit(words: TokWords, vocab: TokVocab) -> np.ndarray:
+    """tip_tok_fit of the words against the vocabulary: int64 [5, k] host columns (first-occurrence key, count,
+    docs, first byte offset, length) of the k distinct words the batch contains, ordered by first occurrence.  A key
+    below vocab.n is that vocabulary entry; a key nv + o is a new word first seen as word o of the batch."""
+    dev = words.text.device
+    nv, n = vocab.n, words.n_words
+    cap, doc_cap = _pow2_at_least(2 * (nv + n)), _pow2_at_least(2 * n)
+    first, count, docs = torch.empty((3, cap), dtype=torch.int64, device=dev)
+    keys = vocab.table(cap, first)
+    doc_keys = torch.empty(doc_cap, dtype=torch.int64, device=dev)
+    out = torch.empty((5, nv + n), dtype=torch.int64, device=dev)
+    n_out = torch.empty(1, dtype=torch.int64, device=dev)
+    _lib.check(_lib.load().tip_tok_fit(_p(words.text), _p(words.start), _p(words.length), _p(words.text_id),
+                                       _p(words.hash), n, _p(vocab.arena), _p(vocab.start), _p(vocab.length),
+                                       _p(vocab.hash), nv, _p(keys), _p(first), _p(count), _p(docs), cap, _p(doc_keys),
+                                       doc_cap, _p(out), nv + n, _p(n_out), _stream()), "tip_tok_fit")
+    cols = out[:, :int(n_out.item())].cpu().numpy()
+    return cols[:, np.argsort(cols[0], kind="stable")]
+
+
+def tok_lookup(words: TokWords, vocab: TokVocab, num_words: int, ragged: bool, maxlen: Optional[int] = None,
+               padding: str = "pre", truncating: str = "pre", value: int = 0):
+    """tip_tok_lookup: (ragged kept ids int32 or None, kept_off int64 [n_texts + 1], padded int32 [n_texts, maxlen]
+    or None) on the device; maxlen None writes no padded rows."""
+    dev = words.text.device
+    keys, cap = vocab.lookup_table()
+    w_id = torch.empty(max(words.n_words, 1), dtype=torch.int32, device=dev)
+    kept_off = torch.empty(words.n_texts + 1, dtype=torch.int64, device=dev)
+    ids = torch.empty(max(words.n_words, 1), dtype=torch.int32, device=dev) if ragged else None
+    padded = None if maxlen is None else torch.empty((words.n_texts, maxlen), dtype=torch.int32, device=dev)
+    _lib.check(_lib.load().tip_tok_lookup(_p(words.text), _p(words.start), _p(words.length), _p(words.hash),
+                                          words.n_words, _p(vocab.arena), _p(vocab.start), _p(vocab.length),
+                                          _p(vocab.hash), _p(vocab.index), vocab.n, _p(keys), cap, num_words,
+                                          _p(words.word_off), words.n_texts, _p(w_id), _p(kept_off), _p(ids),
+                                          _p(padded), 0 if maxlen is None else maxlen, int(padding == "pre"),
+                                          int(truncating == "pre"), value, _stream()), "tip_tok_lookup")
+    return ids, kept_off, padded
