@@ -16,24 +16,12 @@ import numpy as np
 import pytest
 
 from oracle import c_oracle
+from oracle.filter_oracle import _bf16
+from oracle.filter_oracle import threshold_hi as _thr_hi
 
 pytestmark = pytest.mark.gpu
 
 CLS, PER = 4, 1024          # class sizes are multiples of the 128-row train tile, so chunk / tile edges are global
-
-
-def _bf16(a):
-    import torch
-
-    return torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32)).to(torch.bfloat16).to(torch.float32).numpy()
-
-
-def _thr_hi(s, nx, e2, g):
-    """nn_threshold() of csrc/pair_tc.cu at its widest: sqrt.approx 2 ulp high, every float32 rounding against us."""
-    root = np.sqrt(s + g) * (1 + 2.0 ** -21)
-    r = (root + e2) * 1.00004 * (1 + 2.0 ** -22)
-    thr = r * r + g - nx
-    return thr + abs(thr) * 1e-6 + 1e-30 + 2.0 ** -20 * (abs(nx) + r * r)
 
 
 def _descending(rng, dtype):

@@ -9,19 +9,10 @@ import pytest
 
 torch = pytest.importorskip("torch")
 
+from oracle.filter_oracle import _bf16  # noqa: E402
+from oracle.filter_oracle import threshold_lo as _threshold  # noqa: E402
+
 F32 = np.float32
-
-
-def _bf16(a: np.ndarray) -> np.ndarray:
-    return torch.from_numpy(np.ascontiguousarray(a, dtype=F32)).to(torch.bfloat16).to(torch.float32).numpy()
-
-
-def _threshold(s, nx, e2, g):
-    """nn_threshold() of csrc/pair_tc.cu in float32, with sqrt.approx modelled 2 ulp LOW (worst case)."""
-    root = F32(np.sqrt(F32(s + g), dtype=F32)) * F32(1.0 - 2.0 ** -22)
-    r = F32(F32(root + e2) * F32(1.00004))
-    thr = F32(F32(r * r + g) - nx)
-    return F32(thr + F32(abs(thr)) * F32(1e-6) + F32(1e-30))
 
 
 def _check(x, Y, mu, rng):
