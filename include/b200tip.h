@@ -55,6 +55,8 @@
  *   tip_tok_vocab_table ... the vocabulary's hash table
  *   tip_tok_fit         Tokenizer.fit_on_texts: word_counts, first occurrences and word_docs
  *   tip_tok_lookup      Tokenizer.texts_to_sequences and pad_sequences, fused
+ *   tip_keras_adam      case_study_*.py model.fit: Keras' Adam update of every parameter of a model, one launch
+ *   tip_softmax_xent    ... categorical cross-entropy of the softmax output, its gradient and the accuracy count
  */
 #ifndef B200TIP_H
 #define B200TIP_H
@@ -617,6 +619,38 @@ int tip_tok_lookup(const uint8_t* text, const int64_t* w_start, const int32_t* w
                    int64_t num_words, const int64_t* word_off, int64_t n_texts, int32_t* w_id, int64_t* kept_off,
                    int32_t* ragged, int32_t* padded, int64_t maxlen, int pre_padding, int pre_truncating,
                    int32_t value, void* stream);
+
+/* ---- one training step of the case studies' models (case_study_*.py `model.fit`) -------------------------------
+ * One parameter tensor of tip_keras_adam's table: param, its gradient and Adam's two moments, numel float32
+ * elements each, all four laid out alike (element i of one is element i of the others). */
+typedef struct tip_adam_tensor {
+  float* param;
+  const float* grad;
+  float* m;
+  float* v;
+  int64_t numel;
+} tip_adam_tensor;
+
+/* tip_keras_adam: Keras' Adam (TF 2.6 optimizer_v2, amsgrad off, the "epsilon hat" form) over the n_tensors
+ * (1..256) tensors of the DEVICE table, in one launch.  state[2] (device int32): state[0] = steps taken so far,
+ * state[1] = 0 between calls (the kernel's arrival counter).  The step is t = state[0] + 1, and the kernel stores
+ * state[0] = t, so a captured graph replays step after step.  Float32 operation order, each operation rounded
+ * once (no FMA contraction):
+ *   b1t = fl32(beta1 ^ t), b2t = fl32(beta2 ^ t)                (the powers in float64, rounded once)
+ *   lr_t = lr * (sqrt(1 - b2t) / (1 - b1t))
+ *   m = (beta1 * m) + ((1 - beta1) * g)
+ *   v = (beta2 * v) + ((1 - beta2) * (g * g))
+ *   param = param - ((lr_t * m) / (sqrt(v) + epsilon))
+ * total_numel (the table's element count) only sizes the grid; a tensor's elements are read and written by one
+ * thread each, with 16-byte accesses where its four arrays share their alignment.
+ * tip_softmax_xent: the loss head of a step on logits z [rows x classes] (classes 1..32) and targets y (same
+ * shape, float32): *loss = mean over rows of -sum_c y_c log softmax(z)_c, dz (nullable) = (softmax(z) - y) / rows,
+ * *correct = rows whose first argmax of z equals the first argmax of y.  Fixed reduction order: the result
+ * depends on the inputs only. */
+int tip_keras_adam(const tip_adam_tensor* table, int32_t n_tensors, int64_t total_numel, int32_t* state, float lr,
+                   float beta1, float beta2, float epsilon, void* stream);
+int tip_softmax_xent(const float* z, const float* y, int64_t rows, int32_t classes, float* loss, float* dz,
+                     int32_t* correct, void* stream);
 
 /* ---- bring-up / validation: plain accumulator dump ------------------------------------
  * out[256*256] (fp32, row-major, leading dimension 256) = tail-augmented dot products of q rows

@@ -31,6 +31,12 @@ class RerankExtras(C.Structure):
                 ("count_overflow_only", C.c_int32), ("reserved", C.c_int32)]
 
 
+class AdamTensor(C.Structure):
+    """tip_adam_tensor of include/b200tip.h"""
+    _fields_ = [("param", C.c_void_p), ("grad", C.c_void_p), ("m", C.c_void_p), ("v", C.c_void_p),
+                ("numel", C.c_int64)]
+
+
 class WorkItem(C.Structure):
     _fields_ = [("q_row0", C.c_int32), ("q_rows", C.c_int32), ("col0", C.c_int32), ("col1", C.c_int32),
                 ("slot", C.c_int32), ("reserved", C.c_int32)]
@@ -117,6 +123,8 @@ _SIGNATURES = {
                               _i64, _vp, _i64, _vp, _vp]),
     "tip_tok_lookup": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _i64, _i64, _vp, _i64,
                                  _vp, _vp, _vp, _vp, _i64, C.c_int, C.c_int, _i32, _vp]),
+    "tip_keras_adam": (C.c_int, [_vp, _i32, _i64, _vp, _f32, _f32, _f32, _f32, _vp]),
+    "tip_softmax_xent": (C.c_int, [_vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp]),
 }
 
 _lock = threading.Lock()

@@ -2025,3 +2025,53 @@ def tok_lookup(words: TokWords, vocab: TokVocab, num_words: int, ragged: bool, m
                                           _p(padded), 0 if maxlen is None else maxlen, int(padding == "pre"),
                                           int(truncating == "pre"), value, _stream()), "tip_tok_lookup")
     return ids, kept_off, padded
+
+
+# ---- one training step of the case studies' models (train.cu) ----------------------------------------------------
+ADAM_MAX_TENSORS = 256
+
+
+def adam_table(params: Sequence[torch.Tensor], grads: Sequence[torch.Tensor], m: Sequence[torch.Tensor],
+               v: Sequence[torch.Tensor], out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """tip_keras_adam's device table of (param, grad, m, v, numel) rows, as uint8 bytes.  Every tensor is a
+    contiguous float32 CUDA tensor and each row's four share their shape; ValueError otherwise.  `out`: an existing
+    table of the same length to overwrite in place (a captured graph keeps reading it)."""
+    n = len(params)
+    if not 1 <= n <= ADAM_MAX_TENSORS or not len(grads) == len(m) == len(v) == n:
+        raise ValueError(f"tip_keras_adam takes 1..{ADAM_MAX_TENSORS} rows of (param, grad, m, v), got {n}")
+    rows = (_lib.AdamTensor * n)()
+    for i, ts in enumerate(zip(params, grads, m, v)):
+        if any(t.dtype != torch.float32 or not t.is_cuda or not t.is_contiguous() or t.shape != ts[0].shape
+               for t in ts):
+            raise ValueError(f"row {i}: param, grad, m and v must be contiguous float32 CUDA tensors of one shape")
+        rows[i] = _lib.AdamTensor(*(t.data_ptr() for t in ts), ts[0].numel())
+    host = torch.frombuffer(bytearray(rows), dtype=torch.uint8)
+    if out is None:
+        return host.to(params[0].device)
+    out.copy_(host)
+    return out
+
+
+def keras_adam(table: torch.Tensor, n_tensors: int, total_numel: int, state: torch.Tensor, lr: float = 1e-3,
+               beta1: float = 0.9, beta2: float = 0.999, epsilon: float = 1e-7) -> None:
+    """One Keras Adam step over every tensor of an `adam_table` (tip_keras_adam): state is the device int32 [2]
+    (steps taken, 0), advanced by the kernel itself."""
+    if state.dtype != torch.int32 or not state.is_cuda or state.numel() != 2:
+        raise ValueError("state must be a CUDA int32 tensor of 2 elements")
+    lib = _lib.load()
+    _lib.check(lib.tip_keras_adam(_p(table), n_tensors, total_numel, _p(state), lr, beta1, beta2, epsilon, _stream()),
+               "tip_keras_adam")
+
+
+def softmax_xent(z: torch.Tensor, y: torch.Tensor, loss: torch.Tensor, dz: Optional[torch.Tensor],
+                 correct: torch.Tensor) -> None:
+    """tip_softmax_xent into preallocated device outputs: loss (float32, 1 element) = the batch mean of the softmax
+    cross-entropy of logits z [B, C] against targets y [B, C], dz (None: not written) = (softmax(z) - y) / B, correct
+    (int32, 1 element) = rows whose first argmax of z equals that of y."""
+    if z.dim() != 2 or y.shape != z.shape or z.dtype != torch.float32 or y.dtype != torch.float32:
+        raise ValueError(f"z and y must be float32 [B, C] of one shape, got {tuple(z.shape)}, {tuple(y.shape)}")
+    if not (z.is_contiguous() and y.is_contiguous()) or (dz is not None and (dz.shape != z.shape or not dz.is_contiguous())):
+        raise ValueError("z, y and dz must be contiguous")
+    lib = _lib.load()
+    _lib.check(lib.tip_softmax_xent(_p(z), _p(y), z.shape[0], z.shape[1], _p(loss), _p(dz), _p(correct), _stream()),
+               "tip_softmax_xent")
