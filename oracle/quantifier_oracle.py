@@ -17,6 +17,12 @@ Contract (input `p [N, C]`, float32 or float64, C-contiguous; `pred = np.argmax(
   variation_ratio(p)  p [N, S, C]; votes = argmax over C per sample; pred = the lowest class with the most votes
                       (scipy.stats.mode's tie rule); vr = 1 - max_votes / S in float64          uncertainty
 
+NaN follows NumPy, whose functions these are:
+  * pred and every vote are np.argmax's: a NaN beats any number, and the first NaN wins;
+  * max_softmax is NaN on a row with a NaN (np.max propagates it);
+  * pcs is NaN on such a row (np.sort puts NaN last, so s[:, -1] is NaN), and so is the entropy (the sum propagates);
+  * a row with two +inf has pcs inf - inf = NaN; a row of -inf has pcs NaN and max -inf.
+
 `cast_conf_or_unc(as_confidence, scores)` negates a confidence when an uncertainty is asked for (the study calls
 with as_confidence=False, so it stores -max_softmax and -pcs).
 """

@@ -13,8 +13,10 @@ dtype (float64 for VariationRatio).  The quantity is unsigned, as uwiz's `calcul
     VariationRatio             1 - (votes of the mode) / S over S        uncertainty  bit-identical
                                samples [N, S, C]
 
-The prediction is the first argmax of each row; VariationRatio's is the lowest class with the most votes
-(scipy.stats.mode).  The semantics are restated from uncertainty-wizard 0.2.0, which is not a dependency.
+The prediction is np.argmax of each row (the first maximum; the first NaN if the row holds one, and then every
+quantity of the row is NaN); a sample's vote is np.argmax of the sample, and VariationRatio's prediction is the lowest
+class with the most votes (scipy.stats.mode).  The semantics are restated from uncertainty-wizard 0.2.0, which is not
+a dependency.
 """
 from __future__ import annotations
 

@@ -72,6 +72,26 @@ def test_pcs_counts_duplicates_like_a_sort():
     assert np.all(pc[(p == p.max(axis=1, keepdims=True)).sum(axis=1) > 1] == 0)
 
 
+@pytest.mark.parametrize("dt", [np.float32, np.float64])
+def test_nan_rows_follow_numpy(dt):
+    """The NaN rules of the contract: the first NaN is the prediction and the vote, and its row's values are NaN."""
+    nan, inf = np.nan, np.inf
+    p = np.array([[.2, nan, .7, nan], [nan, .1, .2, .3], [.1, .2, .3, nan], [inf, nan, .1, .2],
+                  [nan, nan, nan, nan], [inf, .1, inf, .2], [-inf, -inf, -inf, -inf], [.1, .6, .6, .2]], dtype=dt)
+    want_pred = [1, 0, 3, 1, 0, 0, 0, 1]
+    with np.errstate(invalid="ignore"):
+        for f in (Q.max_softmax, Q.pcs, Q.softmax_entropy):
+            assert np.array_equal(f(p)[0], want_pred), f.__name__
+        mx, pc, ent = Q.max_softmax(p)[1], Q.pcs(p)[1], Q.softmax_entropy(p)[1]
+    assert np.all(np.isnan(mx[:5])) and mx[5] == inf and mx[6] == -inf and mx[7] == dt(.6)
+    assert np.all(np.isnan(pc[:7])) and pc[7] == 0                  # inf - inf and -inf - -inf are NaN too
+    assert np.all(np.isnan(ent[:5])) and np.isnan(ent[6]) and ent[5] == -inf
+    votes = np.broadcast_to(p[:5, None, :], (5, 3, 4))             # three samples of the NaN rows
+    assert np.array_equal(Q.vote_counts(votes).argmax(axis=1), want_pred[:5])
+    pred, vr = Q.variation_ratio(votes)
+    assert np.array_equal(pred, want_pred[:5]) and np.array_equal(vr, np.zeros(5))
+
+
 def test_product_classes_have_the_uwiz_surface():
     from simple_tip_b200.core import quantifiers as P
     from simple_tip_b200.core.deepgini import DeepGini
