@@ -57,6 +57,8 @@
  *   tip_tok_lookup      Tokenizer.texts_to_sequences and pad_sequences, fused
  *   tip_keras_adam      case_study_*.py model.fit: Keras' Adam update of every parameter of a model, one launch
  *   tip_softmax_xent    ... categorical cross-entropy of the softmax output, its gradient and the accuracy count
+ *   tip_softmax_xent_seg  ... the same head for M models trained in one stack, one segment of rows per model
+ *   tip_stack_gather    ... one step's batch for every model of a stack, in one launch
  */
 #ifndef B200TIP_H
 #define B200TIP_H
@@ -651,6 +653,22 @@ int tip_keras_adam(const tip_adam_tensor* table, int32_t n_tensors, int64_t tota
                    float beta1, float beta2, float epsilon, void* stream);
 int tip_softmax_xent(const float* z, const float* y, int64_t rows, int32_t classes, float* loss, float* dz,
                      int32_t* correct, void* stream);
+/* tip_softmax_xent_seg: tip_softmax_xent on each of `segments` consecutive segments of rows_per_segment rows:
+ * segment s (rows [s * rows_per_segment, (s + 1) * rows_per_segment) of z, y and dz) gives loss[s], its dz rows
+ * divided by rows_per_segment and correct[s], bit for bit what tip_softmax_xent gives on that segment alone.
+ * tip_softmax_xent is the launch with one segment. */
+int tip_softmax_xent_seg(const float* z, const float* y, int64_t segments, int64_t rows_per_segment, int32_t classes,
+                         float* loss, float* dz, int32_t* correct, void* stream);
+/* tip_stack_gather: the batch of one step for `models` models trained in one stack.  pool [*, row_elems] (dtype
+ * TIP_F32, TIP_F64 or TIP_I32, contiguous rows); rows [models][n_rows] (int64) = each model's pool rows; perm
+ * [models][n_perm] (int64, values < n_perm <= n_rows) = each model's permutation of its first n_perm rows.  Row j
+ * (j < b) of model m is pool row rows[m][perm[m][start + j]].  channels == 0: out [models][b][row_elems]
+ * (model-major); channels > 0: out [b][P][models][channels] with P = row_elems / channels (an NHWC batch of
+ * models * channels channels).  out is float32 for TIP_F32 and TIP_F64 (rounded to nearest), int32 for TIP_I32.
+ * The pool row indexes are not range-checked here: the caller checks the rows table once. */
+int tip_stack_gather(const void* pool, int32_t dtype, int64_t row_elems, const int64_t* rows, int64_t n_rows,
+                     const int64_t* perm, int64_t n_perm, int64_t start, int64_t b, int64_t models, int64_t channels,
+                     void* out, void* stream);
 
 /* ---- bring-up / validation: plain accumulator dump ------------------------------------
  * out[256*256] (fp32, row-major, leading dimension 256) = tail-augmented dot products of q rows

@@ -125,6 +125,8 @@ _SIGNATURES = {
                                  _vp, _vp, _vp, _vp, _i64, C.c_int, C.c_int, _i32, _vp]),
     "tip_keras_adam": (C.c_int, [_vp, _i32, _i64, _vp, _f32, _f32, _f32, _f32, _vp]),
     "tip_softmax_xent": (C.c_int, [_vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp]),
+    "tip_softmax_xent_seg": (C.c_int, [_vp, _vp, _i64, _i64, _i32, _vp, _vp, _vp, _vp]),
+    "tip_stack_gather": (C.c_int, [_vp, _i32, _i64, _vp, _i64, _vp, _i64, _i64, _i64, _i64, _i64, _vp, _vp]),
 }
 
 _lock = threading.Lock()

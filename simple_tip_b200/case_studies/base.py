@@ -10,7 +10,8 @@ the attention projections [embed, heads, key_dim] / [heads, key_dim, embed]), Co
 
 `CaseStudy` runs the reference's four phases for a torch model — `train`, `run_prio_eval`,
 `run_active_learning_eval`, `collect_activations` — over an output folder, one model after the other (uwiz's
-process pool and its `context` are not part of it).
+process pool and its `context` are not part of it).  `train` and `run_active_learning_eval` can instead train their
+models together in one stack (`stacked=True`, `core.training.fit_stack`), in one process on one GPU.
 """
 from __future__ import annotations
 
@@ -22,7 +23,7 @@ import torch
 import torch.nn.functional as F
 
 from ..core import active_learning, activations, prioritization
-from ..core.training import fit, glorot_limit, uniform_
+from ..core.training import fit, fit_stack, glorot_limit, uniform_
 
 MODELS_FOLDER = "models"
 
@@ -282,6 +283,14 @@ class CaseStudy:
         return fit(self.new_model(), x.to(self.device), y.to(self.device), self.batch_size, self.epochs,
                    validation_split=0.1)
 
+    def stacked_training_process(self, x_pool, y_pool, rows) -> List[KerasSequential]:
+        """The recipe for rows.shape[0] fresh networks trained together (`fit_stack`): network k on
+        x_pool[rows[k]], y_pool[rows[k]] (active learning's `stacked_training_process`)."""
+        dev = self.device
+        models = [self.new_model() for _ in range(rows.shape[0])]
+        return fit_stack(models, x_pool.to(dev), y_pool.to(dev), rows.to(dev), self.batch_size, self.epochs,
+                         validation_split=0.1)
+
     def model_path(self, model_id: int) -> str:
         return model_path(self.output_folder, self.name, model_id)
 
@@ -290,12 +299,17 @@ class CaseStudy:
         return load_state(self.network(), self.model_path(model_id), self.device)
 
     # ---- the four phases ---------------------------------------------------------------------------------------
-    def train(self, model_ids: Sequence[int]) -> None:
-        """`_model_creator` per id (case_study.py:77-92): the recipe on the training set, saved."""
+    def train(self, model_ids: Sequence[int], stacked: bool = False) -> None:
+        """`_model_creator` per id (case_study.py:77-92): the recipe on the training set, saved.  stacked=True trains
+        all ids' models together in one stack (`stacked_training_process`) instead of one after the other."""
         x, y = self.train_set
         y = one_hot(y, self.num_classes, self.device)
-        for model_id in model_ids:
-            model = self.training_process(x, y)
+        if stacked:
+            rows = torch.arange(x.shape[0], dtype=torch.int64, device=self.device).expand(len(model_ids), -1)
+            models = self.stacked_training_process(x, y, rows.contiguous())
+        else:
+            models = (self.training_process(x, y) for _ in model_ids)
+        for model_id, model in zip(model_ids, models):
             path = self.model_path(model_id)
             os.makedirs(os.path.dirname(path), exist_ok=True)
             torch.save(model.state_dict(), path)
@@ -312,16 +326,18 @@ class CaseStudy:
                 batch_size=self.prediction_badge_size)
         return res
 
-    def run_active_learning_eval(self, model_ids: Sequence[int]) -> Dict[int, tuple]:
+    def run_active_learning_eval(self, model_ids: Sequence[int], stacked: bool = False) -> Dict[int, tuple]:
         """`_active_learning_evaluator` per id: `core.active_learning.evaluate` with `training_process` as the
-        retraining; returns {model_id: evaluate's result}."""
+        retraining (stacked=True: a model id's retrainings trained together by `stacked_training_process`); returns
+        {model_id: evaluate's result}."""
         res = {}
         for model_id in model_ids:
             res[model_id] = active_learning.evaluate(
                 model_id, self.name, self.load_model(model_id), self.train_set[0], self.train_set[1],
                 self.nominal_set[0], self.nominal_set[1], self.ood_set[0], self.ood_set[1], self.nc_layers,
                 self.sa_layers, self.training_process, observed_share=0.5, num_selected=self.num_selected,
-                num_classes=self.num_classes, dsa_badge_size=self.dsa_badge_size, output_folder=self.output_folder)
+                num_classes=self.num_classes, dsa_badge_size=self.dsa_badge_size, output_folder=self.output_folder,
+                stacked_training_process=self.stacked_training_process if stacked else None)
         return res
 
     def collect_activations(self, model_ids: Sequence[int]) -> None:

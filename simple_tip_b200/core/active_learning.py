@@ -42,8 +42,9 @@ OUTPUT_FOLDER = "/assets/"        # case_study.py:10
 
 def evaluate(model_id: int, case_study: str, model, train_x, train_y, nominal_test_x, nominal_test_labels,
              ood_test_x, ood_test_labels, nc_activation_layers: Sequence, sa_activation_layers: Sequence,
-             training_process: Callable, observed_share: float, num_selected: int, num_classes: Optional[int],
-             dsa_badge_size: Optional[int] = None, output_folder: str = OUTPUT_FOLDER, batch_size: int = 128
+             training_process: Optional[Callable], observed_share: float, num_selected: int,
+             num_classes: Optional[int], dsa_badge_size: Optional[int] = None, output_folder: str = OUTPUT_FOLDER,
+             batch_size: int = 128, stacked_training_process: Optional[Callable] = None
              ) -> Tuple[SplitEvaluation, MetricSelection, Dict[Tuple[str, str], SplitEvaluation]]:
     """eval_active_learning.py:34-131 for a `torch.nn.Module` whose last output is its softmax.
 
@@ -52,6 +53,14 @@ def evaluate(model_id: int, case_study: str, model, train_x, train_y, nominal_te
     flattened labels; it returns a `torch.nn.Module`.  The layers are as `TransparentModel`'s activation_layers;
     `batch_size` is the badge size of the arms' forward passes and of the accuracy evaluation.  The result files go
     to `{output_folder}/active_learning/` (created when missing).
+
+    `stacked_training_process(x_pool, y_pool, rows)`, when given, retrains every selection's model in one call
+    instead (and `training_process` may be None): x_pool is the training set followed by the nominal and the OOD
+    observed split, concatenated once on the inputs' device (a torch tensor), y_pool their labels the same way (one-hot
+    as above, on x_pool's device), and rows the int64 [selections, n] tensor of pool rows on that device whose row k
+    is exactly the retraining set `training_process` would receive for selection k (`np.random.permutation` is drawn
+    once per selection, in the same order).  It returns the retrained models in selection order, which are then
+    evaluated one by one as the sequential loop evaluates them.
 
     Returns (original model's accuracies, selections, {(metric, "nominal" / "ood"): retrained model's accuracies}),
     each dict in the reference's insertion order; the reference returns None."""
@@ -73,13 +82,20 @@ def evaluate(model_id: int, case_study: str, model, train_x, train_y, nominal_te
     _selection_sanity_checks(num_selected, selections)
 
     active_accuracies: Dict[Tuple[str, str], SplitEvaluation] = dict()
-    for (metric, ood_or_nom), selected_indexes in selections.items():
-        x, y = active_datasets[ood_or_nom, OBS]
-        new_model = _retrain(num_classes, training_process, train_x, train_y, _take(x, selected_indexes),
-                             _take(y, selected_indexes))
-        # every model is evaluated on all four splits, as in the reference (:104-109)
-        active_accuracies[(metric, ood_or_nom)] = _evaluate(new_model, active_datasets, num_classes, batch_size)
-        del new_model
+    if stacked_training_process is not None:
+        new_models = _retrain_stacked(num_classes, stacked_training_process, train_x, train_y, active_datasets,
+                                      selections)
+        for key, new_model in zip(selections, new_models):
+            active_accuracies[key] = _evaluate(new_model, active_datasets, num_classes, batch_size)
+        del new_models, new_model
+    else:
+        for (metric, ood_or_nom), selected_indexes in selections.items():
+            x, y = active_datasets[ood_or_nom, OBS]
+            new_model = _retrain(num_classes, training_process, train_x, train_y, _take(x, selected_indexes),
+                                 _take(y, selected_indexes))
+            # every model is evaluated on all four splits, as in the reference (:104-109)
+            active_accuracies[(metric, ood_or_nom)] = _evaluate(new_model, active_datasets, num_classes, batch_size)
+            del new_model
 
     results.persist_active_learning(output_folder, case_study, model_id, "original", "na", original_model_eval)
     for (metric, ood_or_nom), eval_res in active_accuracies.items():
@@ -159,6 +175,35 @@ def _retrain(num_classes, training_process, train_x, train_y, new_x, new_y):
     if num_classes is not None:
         y = _one_hot(y, num_classes)
     return training_process(x, y)
+
+
+def _retrain_stacked(num_classes, stacked_training_process, train_x, train_y, datasets: SplitDataset,
+                     selections: MetricSelection) -> list:
+    """`_retrain` for every selection in one `stacked_training_process(x_pool, y_pool, rows)` call: the pool is the
+    training set followed by the two observed splits, and rows[k] maps selection k's merged set, shuffled by the
+    same global-RNG draw `_retrain` takes, to pool rows, so x_pool[rows[k]] is what `_retrain` would hand over."""
+    import torch
+
+    assert train_y.shape[0] == np.prod(train_y.shape)
+    x_pool, y_pool, offset = train_x, train_y.reshape(-1), {}
+    n = len(train_x)
+    for name in (NOM, OOD):
+        x, y = datasets[name, OBS]
+        assert y.shape[0] == np.prod(y.shape)
+        offset[name] = n
+        n += len(x)
+        x_pool, y_pool = _concat(x_pool, x), _concat(y_pool, y.reshape(-1))
+    x_pool = _as_tensor(x_pool)
+    y_pool = _as_tensor(y_pool, x_pool.device)
+    if num_classes is not None:
+        y_pool = _one_hot(y_pool, num_classes)
+    train_rows = np.arange(len(train_x), dtype=np.int64)
+    rows = []
+    for (_, ood_or_nom), selected_indexes in selections.items():
+        merged = np.concatenate((train_rows, offset[ood_or_nom] + np.asarray(selected_indexes, dtype=np.int64)))
+        rows.append(merged[np.random.permutation(len(merged))])
+    rows = torch.from_numpy(np.stack(rows)).to(x_pool.device)
+    return list(stacked_training_process(x_pool, y_pool, rows))
 
 
 def _get_random_section(dataset: SplitDataset, num_selected: int) -> MetricSelection:

@@ -1,6 +1,7 @@
-// train.cu — the two kernels of one training step of the case studies' models (case_study_*.py `model.fit`): Keras'
-// Adam update over every parameter of a model in one launch, and the fused softmax cross-entropy head.  Convolutions,
-// GEMMs, pooling, normalisation and attention stay with cuDNN / cuBLAS through torch.
+// train.cu — the kernels of one training step of the case studies' models (case_study_*.py `model.fit`): Keras'
+// Adam update over every parameter of a model in one launch, the fused softmax cross-entropy head (per segment of
+// rows, one segment per model of a stack), and the gather of a step's batch for every model of a stack.
+// Convolutions, GEMMs, pooling, normalisation and attention stay with cuDNN / cuBLAS through torch.
 //
 // tip_keras_adam: one flat index space over all tensors of the table.  A tensor whose param, grad, m and v share
 // their address modulo 16 is walked as a scalar head up to the 16-byte boundary, float4 units, and a scalar tail;
@@ -10,9 +11,13 @@
 // the last block to finish (an arrival counter next to t) stores t + 1 and clears the counter, so a captured graph
 // can be replayed step after step.
 //
-// tip_softmax_xent: one block of 32 warps, warp w takes rows w, w + 32, ...; per row the max, the sums and the
-// argmaxes are fixed xor-shuffle trees, the per-row losses are summed in double in row order per warp and the 32
-// warp sums in a fixed tree, so the result does not depend on anything but the inputs.
+// tip_softmax_xent / tip_softmax_xent_seg: one block of 32 warps per segment of rows (a single segment for
+// tip_softmax_xent), warp w takes the segment's rows w, w + 32, ...; per row the max, the sums and the argmaxes are
+// fixed xor-shuffle trees, the per-row losses are summed in double in row order per warp and the 32 warp sums in a
+// fixed tree, so a segment's result depends on nothing but its own rows.
+//
+// tip_stack_gather: one thread per output element of a stacked batch; row j of model m is pool row
+// rows[m][perm[m][start + j]], written model-major [M, b, R] or channel-interleaved [b, P, M, C] (R = P * C).
 #include "common.cuh"
 
 namespace tip {
@@ -147,11 +152,16 @@ __device__ __forceinline__ int warp_first_argmax(float v, bool live) {
   return hit ? __ffs(hit) - 1 : 0;
 }
 
+// block s: the segment of rows [s * rows, (s + 1) * rows), its loss into loss[s] and its count into correct[s]
 __global__ void __launch_bounds__(kXentWarps * 32) softmax_xent_kernel(const float* __restrict__ z,
                                                                        const float* __restrict__ y, int64_t rows,
                                                                        int classes, float* __restrict__ loss,
                                                                        float* __restrict__ dz,
                                                                        int32_t* __restrict__ correct) {
+  const int64_t seg = blockIdx.x, first = seg * rows * classes;
+  z += first;
+  y += first;
+  if (dz) dz += first;
   __shared__ double part[kXentWarps];
   __shared__ int hits[kXentWarps];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -201,9 +211,38 @@ __global__ void __launch_bounds__(kXentWarps * 32) softmax_xent_kernel(const flo
       h += __shfl_xor_sync(0xffffffffu, h, o);
     }
     if (lane == 0) {
-      *loss = (float)(a / (double)rows);
-      *correct = h;
+      loss[seg] = (float)(a / (double)rows);
+      correct[seg] = h;
     }
+  }
+}
+
+
+// out[m][j][r] (model-major) or out[j][p][m][c] (channel-interleaved, r = p * C + c) = pool[rows[m][perm[m][start + j]]][r]
+template <typename Src, typename Dst>
+__global__ void __launch_bounds__(256) stack_gather_kernel(const Src* __restrict__ pool, int64_t row_elems,
+                                                           const int64_t* __restrict__ rows, int64_t n_rows,
+                                                           const int64_t* __restrict__ perm, int64_t n_perm,
+                                                           int64_t start, int64_t b, int64_t models,
+                                                           int64_t channels, bool interleaved,
+                                                           Dst* __restrict__ out) {
+  const int64_t total = models * b * row_elems;
+  for (int64_t o = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; o < total; o += (int64_t)gridDim.x * blockDim.x) {
+    int64_t m, j, r;
+    if (interleaved) {
+      const int64_t c = o % channels, q = o / channels;
+      m = q % models;
+      const int64_t jp = q / models, pixels = row_elems / channels;
+      j = jp / pixels;
+      r = (jp % pixels) * channels + c;
+    } else {
+      r = o % row_elems;
+      const int64_t q = o / row_elems;
+      j = q % b;
+      m = q / b;
+    }
+    const int64_t row = rows[m * n_rows + perm[m * n_perm + start + j]];
+    out[o] = (Dst)pool[row * row_elems + r];
   }
 }
 
@@ -223,13 +262,48 @@ extern "C" int tip_keras_adam(const tip_adam_tensor* table, int32_t n_tensors, i
   return TIP_OK;
 }
 
-extern "C" int tip_softmax_xent(const float* z, const float* y, int64_t rows, int32_t classes, float* loss, float* dz,
-                                int32_t* correct, void* stream) {
+extern "C" int tip_softmax_xent_seg(const float* z, const float* y, int64_t segments, int64_t rows_per_segment,
+                                    int32_t classes, float* loss, float* dz, int32_t* correct, void* stream) {
   using namespace tip;
-  TIP_REQUIRE(rows >= 1, "at least one row");
+  TIP_REQUIRE(segments >= 1 && segments <= INT32_MAX, "1..2^31-1 segments");
+  TIP_REQUIRE(rows_per_segment >= 1, "at least one row per segment");
   TIP_REQUIRE(classes >= 1 && classes <= 32, "1..32 classes");
   TIP_REQUIRE(z && y && loss && correct, "null pointer");
-  softmax_xent_kernel<<<1, kXentWarps * 32, 0, (cudaStream_t)stream>>>(z, y, rows, classes, loss, dz, correct);
+  softmax_xent_kernel<<<(unsigned)segments, kXentWarps * 32, 0, (cudaStream_t)stream>>>(z, y, rows_per_segment, classes,
+                                                                                      loss, dz, correct);
+  TIP_LAUNCH_CHECK();
+  return TIP_OK;
+}
+
+extern "C" int tip_softmax_xent(const float* z, const float* y, int64_t rows, int32_t classes, float* loss, float* dz,
+                                int32_t* correct, void* stream) {
+  return tip_softmax_xent_seg(z, y, 1, rows, classes, loss, dz, correct, stream);
+}
+
+extern "C" int tip_stack_gather(const void* pool, int32_t dtype, int64_t row_elems,
+                                const int64_t* rows, int64_t n_rows, const int64_t* perm, int64_t n_perm,
+                                int64_t start, int64_t b, int64_t models, int64_t channels, void* out, void* stream) {
+  using namespace tip;
+  TIP_REQUIRE(dtype == TIP_F32 || dtype == TIP_F64 || dtype == TIP_I32, "float32, float64 or int32 pool");
+  TIP_REQUIRE(row_elems >= 1 && models >= 1 && b >= 1, "empty rows or batch");
+  TIP_REQUIRE(n_perm >= 1 && n_perm <= n_rows, "perm indexes the first n_perm of each model's n_rows rows");
+  TIP_REQUIRE(start >= 0 && start + b <= n_perm, "batch [start, start + b) within the permutation");
+  TIP_REQUIRE(channels >= 0 && (channels == 0 || row_elems % channels == 0), "row_elems is pixels x channels");
+  TIP_REQUIRE(pool && rows && perm && out, "null pointer");
+  const bool interleaved = channels > 0;
+  const int64_t total = models * b * row_elems;
+  const int grid = (int)max((int64_t)1, min((total + 255) / 256, (int64_t)sm_count() * 16));
+  cudaStream_t s = (cudaStream_t)stream;
+  if (dtype == TIP_F32)
+    stack_gather_kernel<float, float><<<grid, 256, 0, s>>>((const float*)pool, row_elems, rows, n_rows, perm, n_perm,
+                                                            start, b, models, channels, interleaved, (float*)out);
+  else if (dtype == TIP_F64)
+    stack_gather_kernel<double, float><<<grid, 256, 0, s>>>((const double*)pool, row_elems, rows, n_rows, perm, n_perm,
+                                                             start, b, models, channels, interleaved, (float*)out);
+  else
+    stack_gather_kernel<int32_t, int32_t><<<grid, 256, 0, s>>>((const int32_t*)pool, row_elems, rows, n_rows, perm,
+                                                                n_perm, start, b, models, channels, interleaved,
+                                                                (int32_t*)out);
   TIP_LAUNCH_CHECK();
   return TIP_OK;
 }

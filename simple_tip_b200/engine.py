@@ -2075,3 +2075,75 @@ def softmax_xent(z: torch.Tensor, y: torch.Tensor, loss: torch.Tensor, dz: Optio
     lib = _lib.load()
     _lib.check(lib.tip_softmax_xent(_p(z), _p(y), z.shape[0], z.shape[1], _p(loss), _p(dz), _p(correct), _stream()),
                "tip_softmax_xent")
+
+
+def softmax_xent_seg(z: torch.Tensor, y: torch.Tensor, loss: torch.Tensor, dz: Optional[torch.Tensor],
+                     correct: torch.Tensor) -> None:
+    """tip_softmax_xent_seg: `softmax_xent` on each of the M segments of logits z [M, B, C] against targets y
+    [M, B, C]: loss (float32 [M]), dz (None: not written; else [M, B, C], each segment divided by B) and correct
+    (int32 [M]), segment s bit for bit what `softmax_xent(z[s], y[s], ...)` gives."""
+    if z.dim() != 3 or y.shape != z.shape or z.dtype != torch.float32 or y.dtype != torch.float32:
+        raise ValueError(f"z and y must be float32 [M, B, C] of one shape, got {tuple(z.shape)}, {tuple(y.shape)}")
+    if not (z.is_contiguous() and y.is_contiguous()) or (dz is not None and (dz.shape != z.shape or not dz.is_contiguous())):
+        raise ValueError("z, y and dz must be contiguous")
+    m = z.shape[0]
+    if loss.numel() < m or correct.numel() < m or loss.dtype != torch.float32 or correct.dtype != torch.int32:
+        raise ValueError(f"loss (float32) and correct (int32) need {m} elements")
+    lib = _lib.load()
+    _lib.check(lib.tip_softmax_xent_seg(_p(z), _p(y), m, z.shape[1], z.shape[2], _p(loss), _p(dz), _p(correct),
+                                        _stream()), "tip_softmax_xent_seg")
+
+
+_GATHER_DTYPES = {torch.float32: (_lib.TIP_F32, torch.float32), torch.float64: (_lib.TIP_F64, torch.float32),
+                  torch.int32: (_lib.TIP_I32, torch.int32)}
+
+
+def check_stack_rows(rows: torch.Tensor, pool_rows: int) -> None:
+    """ValueError unless `rows` is a contiguous int64 [M, n] CUDA table of indexes into a pool of `pool_rows` rows
+    (one device-to-host read; `stack_gather` relies on it and does not check per step)."""
+    if rows.dim() != 2 or rows.dtype != torch.int64 or not rows.is_cuda or not rows.is_contiguous() or rows.numel() == 0:
+        raise ValueError(f"rows must be a non-empty contiguous int64 [M, n] CUDA tensor, got {tuple(rows.shape)} "
+                         f"{rows.dtype}")
+    lo, hi = torch.aminmax(rows)
+    lo, hi = int(lo.item()), int(hi.item())
+    if lo < 0 or hi >= pool_rows:
+        raise ValueError(f"rows index [{lo}, {hi}] outside the pool's {pool_rows} rows")
+
+
+def stack_gather(pool: torch.Tensor, rows: torch.Tensor, perm: torch.Tensor, start: int, b: int,
+                 interleaved: bool = False, out: Optional[torch.Tensor] = None, check: bool = True) -> torch.Tensor:
+    """tip_stack_gather: row j < b of model m is `pool[rows[m, perm[m, start + j]]]`, for every model of the rows
+    table [M, n] at once (perm [M, n_perm], int64, a permutation of each model's first n_perm rows).
+
+    pool [N, ...] float32, float64 (gathered as float32) or int32 on the device; any other dtype is refused.
+    interleaved=False: out [M, b, *row_shape] (model-major); True: a pool of NHWC rows [N, H, W, C] gives out
+    [b, H, W, M * C], channel m * C + c of it being model m's channel c.  check=True checks the rows table against
+    the pool (`check_stack_rows`, a device-to-host read); a caller that already did passes False."""
+    if pool.dtype not in _GATHER_DTYPES:
+        raise ValueError(f"tip_stack_gather gathers float32, float64 or int32 pools, not {pool.dtype}")
+    if not pool.is_cuda or not pool.is_contiguous() or pool.dim() < 2:
+        raise ValueError("pool must be a contiguous CUDA tensor [N, ...]")
+    if check:
+        check_stack_rows(rows, pool.shape[0])
+    if perm.dim() != 2 or perm.dtype != torch.int64 or not perm.is_contiguous() or perm.shape[0] != rows.shape[0]:
+        raise ValueError(f"perm must be a contiguous int64 [{rows.shape[0]}, n_perm] tensor, got {tuple(perm.shape)}")
+    m, n_rows = rows.shape
+    n_perm = perm.shape[1]
+    if not (0 <= start and b >= 1 and start + b <= n_perm <= n_rows):
+        raise ValueError(f"batch [{start}, {start + b}) outside a permutation of {n_perm} of {n_rows} rows")
+    dtype, out_dtype = _GATHER_DTYPES[pool.dtype]
+    row_shape = tuple(pool.shape[1:])
+    if interleaved:
+        if pool.dim() != 4:
+            raise ValueError(f"the interleaved layout takes NHWC rows [N, H, W, C], got {tuple(pool.shape)}")
+        shape, channels = (b, *row_shape[:-1], m * row_shape[-1]), row_shape[-1]
+    else:
+        shape, channels = (m, b, *row_shape), 0
+    if out is None:
+        out = torch.empty(shape, dtype=out_dtype, device=pool.device)
+    elif tuple(out.shape) != shape or out.dtype != out_dtype or not out.is_contiguous():
+        raise ValueError(f"out must be contiguous {out_dtype} {shape}")
+    row_elems = int(np.prod(row_shape))
+    _lib.check(_lib.load().tip_stack_gather(_p(pool), dtype, row_elems, _p(rows), n_rows, _p(perm), n_perm, start, b,
+                                            m, channels, _p(out), _stream()), "tip_stack_gather")
+    return out
