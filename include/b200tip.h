@@ -59,6 +59,8 @@
  *   tip_softmax_xent    ... categorical cross-entropy of the softmax output, its gradient and the accuracy count
  *   tip_softmax_xent_seg  ... the same head for M models trained in one stack, one segment of rows per model
  *   tip_stack_gather    ... one step's batch for every model of a stack, in one launch
+ *   tip_mc_head         handler_model.py get_pred_and_uncertainty: MC-dropout samples of a model's dropout head
+ *                       (dropout masks, dense layers and softmax) from its trunk activations, in one launch
  */
 #ifndef B200TIP_H
 #define B200TIP_H
@@ -669,6 +671,38 @@ int tip_softmax_xent_seg(const float* z, const float* y, int64_t segments, int64
 int tip_stack_gather(const void* pool, int32_t dtype, int64_t row_elems, const int64_t* rows, int64_t n_rows,
                      const int64_t* perm, int64_t n_perm, int64_t start, int64_t b, int64_t models, int64_t channels,
                      void* out, void* stream);
+
+/* ---- MC-dropout head: the samples of a model's top-level dropout / dense chain ---------------------------
+ * One layer of the head: a dropout of rate p on its input (p = 0: none), then the dense layer
+ * y = act(x K + b) with K [in][out] (Keras' layout) and b [out], float32, contiguous, on the device. */
+typedef enum tip_mc_activation { TIP_MC_LINEAR = 0, TIP_MC_RELU = 1, TIP_MC_SOFTMAX = 2 } tip_mc_activation;
+typedef enum tip_mc_mode { TIP_MC_OUTPUT = 0, TIP_MC_PREACT = 1 } tip_mc_mode;
+typedef struct tip_mc_layer {
+  const float* kernel;     /* [in][out] */
+  const float* bias;       /* [out] */
+  double p;                /* dropout rate on the layer's input, 0 <= p <= 1 */
+  int32_t in, out;         /* layer 0: 1 <= in <= 8192; later layers: in = the previous out; 1 <= out <= 64 */
+  int32_t activation;      /* tip_mc_activation; TIP_MC_SOFTMAX only on the last layer */
+  int32_t reserved;        /* 0 */
+} tip_mc_layer;
+/* tip_mc_head: h [rows][ld] float32 (the first `in` columns of each row are the trunk activations; row i is the
+ * global row row0 + i); layers [n_layers] (1..4, host memory).  For every row i < rows and sample s < samples,
+ * out[(i * samples + s) * C + c] (C = the last layer's out) receives the last layer's output (mode TIP_MC_OUTPUT)
+ * or its pre-activation x K + b (TIP_MC_PREACT, for tests) for the global sample sample0 + s.
+ *
+ * Arithmetic (restatable bit for bit):
+ *   key(l, r, s) = mix(mix(mix(mix(seed) ^ l) ^ r) ^ s), mix = one splitmix64 step, l = the layer's index in
+ *     `layers`, r = row0 + i, s = sample0 + s;
+ *   u(l, r, s, j) = the low (j even) or high (j odd) 32 bits of mix(key(l, r, s) ^ (j >> 1)) for input unit j;
+ *   unit j is dropped iff u < t, t = rint(p * 2^32) (p = 1 drops every unit);
+ *   x'_j = 0 if dropped, else x_j * scale rounded once, scale = float32(1 / float32(1 - p)) (torch's dropout);
+ *   z_c = ((...((0 + x'_0 K[0][c]) + x'_1 K[1][c]) + ...) + x'_{in-1} K[in-1][c]) + b[c], every product and sum
+ *     rounded once to float32 (no FMA), units in ascending order;
+ *   relu: z < 0 ? 0 : z (NaN stays NaN); softmax: m = max_c z_c, e_c = expf(z_c - m), s = sum of e_c in class
+ *     order, y_c = e_c / s.
+ * The draws depend on (seed, l, r, s, j) only: not on the launch shape, the row split or the sample split. */
+int tip_mc_head(const float* h, int64_t rows, int64_t ld, int64_t row0, int64_t sample0, int64_t samples,
+                const tip_mc_layer* layers, int32_t n_layers, uint64_t seed, int32_t mode, float* out, void* stream);
 
 /* ---- bring-up / validation: plain accumulator dump ------------------------------------
  * out[256*256] (fp32, row-major, leading dimension 256) = tail-augmented dot products of q rows

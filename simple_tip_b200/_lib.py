@@ -21,6 +21,8 @@ ROLE_QUERY, ROLE_TRAIN = 0, 1
 RANGE_SAME_CLASS, RANGE_OTHER_CLASSES = 0, 1
 ROW_TILE, COL_TILE = 128, 256
 STAT_GINI, STAT_MAX, STAT_PCS, STAT_ENTROPY = 0, 1, 2, 3
+MC_LINEAR, MC_RELU, MC_SOFTMAX = 0, 1, 2
+MC_OUTPUT, MC_PREACT = 0, 1
 
 
 class RerankExtras(C.Structure):
@@ -35,6 +37,12 @@ class AdamTensor(C.Structure):
     """tip_adam_tensor of include/b200tip.h"""
     _fields_ = [("param", C.c_void_p), ("grad", C.c_void_p), ("m", C.c_void_p), ("v", C.c_void_p),
                 ("numel", C.c_int64)]
+
+
+class McLayer(C.Structure):
+    """tip_mc_layer of include/b200tip.h"""
+    _fields_ = [("kernel", C.c_void_p), ("bias", C.c_void_p), ("p", C.c_double), ("in_", C.c_int32),
+                ("out", C.c_int32), ("activation", C.c_int32), ("reserved", C.c_int32)]
 
 
 class WorkItem(C.Structure):
@@ -127,6 +135,7 @@ _SIGNATURES = {
     "tip_softmax_xent": (C.c_int, [_vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp]),
     "tip_softmax_xent_seg": (C.c_int, [_vp, _vp, _i64, _i64, _i32, _vp, _vp, _vp, _vp]),
     "tip_stack_gather": (C.c_int, [_vp, _i32, _i64, _vp, _i64, _vp, _i64, _i64, _i64, _i64, _i64, _vp, _vp]),
+    "tip_mc_head": (C.c_int, [_vp, _i64, _i64, _i64, _i64, _i64, _vp, _i32, _u64, _i32, _vp, _vp]),
 }
 
 _lock = threading.Lock()

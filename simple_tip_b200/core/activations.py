@@ -16,7 +16,7 @@ labels in `.../labels/badge_<b>.npy`).  Here the same two things for a `torch.nn
 from __future__ import annotations
 
 import os
-from typing import Dict, Generator, Iterable, List, Optional, Sequence, Tuple, Union
+from typing import Dict, Generator, Iterable, List, NamedTuple, Optional, Sequence, Tuple, Union
 
 import numpy as np
 
@@ -126,9 +126,112 @@ class HookedModelHandler:
 
 DROPOUT_SAMPLE_SIZE = 200      # handler_model.py:7
 MC_ROWS_PER_PASS = 8192        # rows of one MC-dropout forward pass: a batch is replicated up to this many
+MC_SAMPLERS = ("torch", "head")
 
 
-def get_pred_and_uncertainty(model, x, batch_size: int = 32, sample_size: int = DROPOUT_SAMPLE_SIZE, seed: int = 0
+class HeadLayer(NamedTuple):
+    """One dense layer of an MC-dropout head: the dropout rate on its input (0: none), the module(s) it came from,
+    and its activation (None, "relu" or "softmax")."""
+    p: float
+    module: object
+    activation: Optional[str]
+
+
+def mc_head_layers(model) -> Tuple[int, List[HeadLayer]]:
+    """The model's MC-dropout head as `sampler="head"` samples it: (index of the first top-level dropout child, the
+    dense layers from there on).  Like uncertainty-wizard's `stochastic_from_keras`, only the top-level dropout
+    layers are stochastic; dropouts nested inside earlier children stay in eval mode.
+
+    The model must be a `torch.nn.Sequential`; from its first `_DropoutNd` child on, every child must be a
+    `torch.nn.Dropout`, a case-study `Dense` (activation None, "relu" or "softmax"), or a `torch.nn.Linear`
+    optionally followed by `ReLU` or `Softmax(dim=-1 or 1)`; at most one dropout precedes a dense layer, the head
+    ends in a dense layer, and a softmax ends it.  Anything else raises ValueError naming the module.  (-1, []) when
+    the model has no dropout module at all."""
+    import torch
+    from torch.nn.modules.dropout import _DropoutNd
+
+    from ..case_studies.base import Dense
+
+    if not isinstance(model, torch.nn.Sequential):
+        raise ValueError(f"sampler='head' needs a torch.nn.Sequential model, got {type(model).__name__}")
+    children = list(model.children())
+    first = next((i for i, m in enumerate(children) if isinstance(m, _DropoutNd)), -1)
+    if first < 0:
+        if any(isinstance(m, _DropoutNd) for m in model.modules()):
+            raise ValueError("sampler='head' samples top-level dropout layers; this model's dropouts are all nested")
+        return -1, []
+    layers: List[HeadLayer] = []
+    p = None
+    i = first
+    while i < len(children):
+        m = children[i]
+        where = f"child {i} ({type(m).__name__})"
+        if layers and layers[-1].activation == "softmax":
+            raise ValueError(f"sampler='head': {where} follows the head's softmax")
+        if type(m) is torch.nn.Dropout:
+            if p is not None:
+                raise ValueError(f"sampler='head': {where} is a second dropout before one dense layer")
+            p = float(m.p)
+        elif isinstance(m, Dense):
+            if m.activation not in (None, "relu", "softmax"):
+                raise ValueError(f"sampler='head': {where} has activation {m.activation!r}")
+            layers.append(HeadLayer(p or 0.0, m, m.activation))
+            p = None
+        elif type(m) is torch.nn.Linear:
+            act, nxt = None, children[i + 1] if i + 1 < len(children) else None
+            if type(nxt) is torch.nn.ReLU:
+                act = "relu"
+            elif type(nxt) is torch.nn.Softmax and nxt.dim in (-1, 1):
+                act = "softmax"
+            layers.append(HeadLayer(p or 0.0, m, act))
+            p = None
+            i += act is not None
+        else:
+            raise ValueError(f"sampler='head' cannot sample {where}: the head after the first top-level dropout may "
+                             "hold only Dropout, Dense and Linear (+ ReLU / Softmax) layers")
+        i += 1
+    if p is not None or not layers:
+        raise ValueError("sampler='head': the head must end in a dense layer")
+    if len(layers) > 4:
+        raise ValueError(f"sampler='head' samples heads of at most 4 dense layers, this one has {len(layers)}")
+    return first, layers
+
+
+def _head_tensors(layers: Sequence[HeadLayer], dev):
+    """(kernel [in, out], bias [out], p, activation) per layer as contiguous float32 on dev; Linear weights are
+    transposed once."""
+    import torch
+
+    out = []
+    for layer in layers:
+        m = layer.module
+        if isinstance(m, torch.nn.Linear):
+            kernel = m.weight.detach().t()
+            bias = m.bias.detach() if m.bias is not None else torch.zeros(m.out_features, device=m.weight.device)
+        else:
+            kernel, bias = m.kernel.detach(), m.bias.detach()
+        out.append((kernel.to(dev, torch.float32).contiguous(), bias.to(dev, torch.float32).contiguous(), layer.p,
+                    layer.activation))
+    return out
+
+
+def head_input(trunk: Sequence, n: int):
+    """The head's input captured batch by batch in the point pass, as one [n, D] tensor; ValueError unless every
+    batch is 2-D float32 (a head of dense layers takes flat rows) and they hold n rows together."""
+    import torch
+
+    for t in trunk:
+        if t.dim() != 2 or t.dtype != torch.float32:
+            raise ValueError(f"sampler='head' needs the head's input as 2-D float32 [N, D], got {tuple(t.shape)} "
+                             f"{t.dtype}")
+    h = torch.cat(list(trunk), dim=0) if len(trunk) != 1 else trunk[0]
+    if h.shape[0] != n:
+        raise ValueError(f"the head saw {h.shape[0]} rows, the model's output has {n}")
+    return h
+
+
+def get_pred_and_uncertainty(model, x, batch_size: int = 32, sample_size: int = DROPOUT_SAMPLE_SIZE, seed: int = 0,
+                             sampler: Optional[str] = None
                              ) -> Tuple[np.ndarray, Dict[str, np.ndarray], Dict[str, List[float]]]:
     """Point predictions and uncertainties of a torch model (handler_model.py:102-173, `BaseModel.get_pred_and_uncertainty`).
 
@@ -153,7 +256,15 @@ def get_pred_and_uncertainty(model, x, batch_size: int = 32, sample_size: int = 
     3.9 GB before any activation; for large inputs pass a smaller `batch_size`, or a `sample_size` that keeps
     batch_size x sample_size small (a batch is never split, so batch_size rows is the floor).  The passes draw
     from torch's RNG seeded with `seed` inside `torch.random.fork_rng` (forking only the host's and the model
-    device's state), so results repeat and the caller's RNG state is untouched."""
+    device's state), so results repeat and the caller's RNG state is untouched.
+
+    sampler: None reads the B200TIP_MC environment variable, default "torch" (the MC-dropout passes above).
+    "head" samples only the model's head from its first top-level dropout child on (`mc_head_layers`; ValueError
+    for a model it cannot sample, before any work): the point pass captures the head's input (2-D float32 [N, D]),
+    and `tip_mc_head` draws the masks and runs the dense layers for all `sample_size` samples of MC_ROWS_PER_PASS
+    rows per launch, fed to the same vote kernels.  Its masks are this library's counter-based draws keyed by
+    (seed, layer, row, sample, unit), not torch's, and dropouts nested in the trunk (the IMDB transformer block's)
+    are not sampled, as in uncertainty-wizard; times["VR"] = [0, head-kernel time, vote time, 0]."""
     import torch
     from torch.nn.modules.dropout import _DropoutNd
 
@@ -162,6 +273,10 @@ def get_pred_and_uncertainty(model, x, batch_size: int = 32, sample_size: int = 
     from .timer import Timer
     from .. import engine as E
 
+    sampler = sampler if sampler is not None else os.environ.get("B200TIP_MC", "torch")
+    if sampler not in MC_SAMPLERS:
+        raise ValueError(f"sampler must be one of {MC_SAMPLERS}, got {sampler!r}")
+    head_at, head = mc_head_layers(model) if sampler == "head" else (-1, [])
     score_dev = E.require_cuda()
     dev = next(iter(model.parameters()), torch.empty(0)).device
     if not isinstance(x, torch.Tensor):
@@ -181,10 +296,17 @@ def get_pred_and_uncertainty(model, x, batch_size: int = 32, sample_size: int = 
     modes = [(m, m.training) for m in model.modules()]
     uncertainties: Dict[str, np.ndarray] = {}
     times: Dict[str, List[float]] = {}
+    trunk: List[torch.Tensor] = []
+    hook = (list(model.children())[head_at].register_forward_pre_hook(lambda _m, inp: trunk.append(inp[0].detach()))
+            if head else None)
     try:
         pred_timer = Timer()
-        probs = synced(lambda: TransparentModel(model, [], include_last_layer=True).collect(x, batch_size)[0],
-                       pred_timer)
+        try:
+            probs = synced(lambda: TransparentModel(model, [], include_last_layer=True).collect(x, batch_size)[0],
+                           pred_timer)
+        finally:
+            if hook is not None:
+                hook.remove()
         pred = None
         for q in (Q.MaxSoftmax, Q.PredictionConfidenceScore, Q.SoftmaxEntropy, DeepGini):
             timer = Timer()
@@ -196,7 +318,24 @@ def get_pred_and_uncertainty(model, x, batch_size: int = 32, sample_size: int = 
             times[name] = [0, pred_timer.get(), timer.get(), 0]
 
         dropouts = [m for m in model.modules() if isinstance(m, _DropoutNd)]
-        if dropouts:
+        if head:
+            h = E.to_device(head_input(trunk, probs.shape[0]), score_dev)
+            n, c = probs.shape
+            layers = _head_tensors(head, score_dev)
+            votes = Q.Votes(n, c, score_dev)
+            head_timer, vote_timer = Timer(), Timer()
+            for start in range(0, n if sample_size >= 1 else 0, MC_ROWS_PER_PASS):
+                b = min(MC_ROWS_PER_PASS, n - start)
+                out = synced(lambda: E.mc_head(h[start:start + b], layers, seed, sample_size, row0=start),
+                             head_timer)
+                if out.shape[2] != c:
+                    raise ValueError(f"the head gives {out.shape[2]} classes, the model's output {c}")
+                synced(lambda: votes.add(out, sample_size, sample_stride=c, row_stride=sample_size * c, row0=start,
+                                         rows=b), vote_timer)
+            _, vr = synced(lambda: votes.finish(sample_size), vote_timer)
+            uncertainties["VR"] = vr
+            times["VR"] = [0, head_timer.get(), vote_timer.get(), 0]
+        elif dropouts:
             n, c = probs.shape
             votes = Q.Votes(n, c, score_dev)
             sampling_timer, vote_timer = Timer(), Timer()

@@ -39,6 +39,14 @@ void count_launch(int n = 1);
 
 int sm_count();
 
+// ---- counter-based RNG: one splitmix64 step; a key (seed, k1, k2, ...) is hashed as mix(...mix(mix(seed) ^ k1) ^ k2...)
+__host__ __device__ __forceinline__ uint64_t km_mix(uint64_t z) {
+  z += 0x9E3779B97F4A7C15ull;
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+
 // ---- IEEE arithmetic without FMA contraction (NumPy never fuses) --------------------------
 template <typename T> struct Rn;
 template <> struct Rn<float> {

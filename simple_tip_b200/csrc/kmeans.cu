@@ -24,13 +24,7 @@ constexpr int64_t kKmPartBudget = 256ll << 20;  // bytes of per-block centre sum
 
 enum { KM_ACTIVE = 0, KM_STRICT = 1, KM_TOL = 2, KM_MAXITER = 3 };
 
-// ---- counter-based RNG: splitmix64 over the key (seed, k, run, step, trial) ------------------------------------
-__host__ __device__ __forceinline__ uint64_t km_mix(uint64_t z) {
-  z += 0x9E3779B97F4A7C15ull;
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  return z ^ (z >> 31);
-}
+// ---- counter-based RNG: splitmix64 (km_mix, common.cuh) over the key (seed, k, run, step, trial) -------------
 __device__ __forceinline__ double km_uniform(uint64_t seed, int k, int run, int step, int trial) {
   uint64_t h = km_mix(seed);
   h = km_mix(h ^ (uint64_t)k);

@@ -2147,3 +2147,61 @@ def stack_gather(pool: torch.Tensor, rows: torch.Tensor, perm: torch.Tensor, sta
     _lib.check(_lib.load().tip_stack_gather(_p(pool), dtype, row_elems, _p(rows), n_rows, _p(perm), n_perm, start, b,
                                             m, channels, _p(out), _stream()), "tip_stack_gather")
     return out
+
+
+MC_MAX_LAYERS = 4         # dense layers of an MC-dropout head
+MC_MAX_IN = 8192          # the head's input width (the trunk's)
+MC_MAX_WIDTH = 64         # units of every head layer
+MC_ACTIVATIONS = {None: _lib.MC_LINEAR, "linear": _lib.MC_LINEAR, "relu": _lib.MC_RELU, "softmax": _lib.MC_SOFTMAX}
+
+
+def mc_head(h: torch.Tensor, layers, seed: int, samples: int, row0: int = 0, sample0: int = 0,
+            out: Optional[torch.Tensor] = None, preact: bool = False) -> torch.Tensor:
+    """tip_mc_head: `samples` MC-dropout samples of a dense head for every row of the trunk activations h
+    [rows, D] (float32 on the current CUDA device, unit column stride, any row stride).  layers: 1..4 tuples
+    (kernel [in, out], bias [out], p, activation), kernel and bias contiguous float32 on h's device, p the dropout
+    rate on the layer's input (0: none), activation None / "linear" / "relu" / "softmax" (softmax only last);
+    D <= 8192, every out <= 64.  Row i of h is global row row0 + i and sample s global sample sample0 + s: the masks
+    depend on (seed, layer, global row, global sample, unit) only (include/b200tip.h).  Returns out [rows, samples,
+    C] float32: the last layer's output, or its pre-activation (preact=True).  Raises ValueError before any launch
+    for anything else."""
+    dev = require_cuda()
+    if not isinstance(h, torch.Tensor) or h.dim() != 2 or h.dtype != torch.float32 or h.device != dev:
+        raise ValueError(f"h must be a 2-D float32 tensor on {dev}, got "
+                         f"{tuple(h.shape) if isinstance(h, torch.Tensor) else type(h).__name__}")
+    if h.shape[0] > 0 and h.shape[1] > 1 and h.stride(1) != 1:
+        raise ValueError("h must have a unit column stride")
+    if not 1 <= len(layers) <= MC_MAX_LAYERS:
+        raise ValueError(f"an MC-dropout head has 1..{MC_MAX_LAYERS} dense layers, got {len(layers)}")
+    if samples < 1 or row0 < 0 or sample0 < 0:
+        raise ValueError(f"samples >= 1, row0 >= 0 and sample0 >= 0, got {samples}, {row0}, {sample0}")
+    table = (_lib.McLayer * len(layers))()
+    width = h.shape[1]
+    if not 1 <= width <= MC_MAX_IN:
+        raise ValueError(f"the head's input width must be 1..{MC_MAX_IN}, got {width}")
+    for i, (kernel, bias, p, act) in enumerate(layers):
+        if act not in MC_ACTIVATIONS or (act == "softmax" and i != len(layers) - 1):
+            raise ValueError(f"layer {i}: activation {act!r} (linear, relu, or softmax on the last layer)")
+        for name, t, dim in (("kernel", kernel, 2), ("bias", bias, 1)):
+            if (not isinstance(t, torch.Tensor) or t.dim() != dim or t.dtype != torch.float32 or t.device != dev
+                    or not t.is_contiguous()):
+                raise ValueError(f"layer {i}: {name} must be a contiguous {dim}-D float32 tensor on {dev}")
+        if kernel.shape[0] != width or not 1 <= kernel.shape[1] <= MC_MAX_WIDTH or tuple(bias.shape) != (kernel.shape[1],):
+            raise ValueError(f"layer {i}: kernel {tuple(kernel.shape)} / bias {tuple(bias.shape)} do not take {width} "
+                             f"inputs to 1..{MC_MAX_WIDTH} units")
+        p = float(p)
+        if not 0.0 <= p <= 1.0:
+            raise ValueError(f"layer {i}: dropout rate {p} outside [0, 1]")
+        table[i] = _lib.McLayer(kernel.data_ptr(), bias.data_ptr(), p, width, kernel.shape[1], MC_ACTIVATIONS[act], 0)
+        width = kernel.shape[1]
+    rows = h.shape[0]
+    shape = (rows, samples, width)
+    if out is None:
+        out = torch.empty(shape, dtype=torch.float32, device=dev)
+    elif tuple(out.shape) != shape or out.dtype != torch.float32 or out.device != dev or not out.is_contiguous():
+        raise ValueError(f"out must be a contiguous float32 {shape} tensor on {dev}")
+    ld = h.stride(0) if rows > 1 else h.shape[1]
+    _lib.check(_lib.load().tip_mc_head(_p(h), rows, ld, row0, sample0, samples, table, len(layers),
+                                       int(seed) & 0xFFFFFFFFFFFFFFFF, _lib.MC_PREACT if preact else _lib.MC_OUTPUT,
+                                       _p(out), _stream()), "tip_mc_head")
+    return out
