@@ -55,6 +55,8 @@
  *   tip_tok_vocab_table ... the vocabulary's hash table
  *   tip_tok_fit         Tokenizer.fit_on_texts: word_counts, first occurrences and word_docs
  *   tip_tok_lookup      Tokenizer.texts_to_sequences and pad_sequences, fused
+ *   tip_corrupt_*       src/core/text_corruptor.py:311-508 TextCorruptor.corrupt: the split, MD5 seeds, NumPy's PCG64
+ *                       draws and the four corruptions, string for string
  *   tip_keras_adam      case_study_*.py model.fit: Keras' Adam update of every parameter of a model, one launch
  *   tip_softmax_xent    ... categorical cross-entropy of the softmax output, its gradient and the accuracy count
  *   tip_softmax_xent_seg  ... the same head for M models trained in one stack, one segment of rows per model
@@ -623,6 +625,84 @@ int tip_tok_lookup(const uint8_t* text, const int64_t* w_start, const int32_t* w
                    int64_t num_words, const int64_t* word_off, int64_t n_texts, int32_t* w_id, int64_t* kept_off,
                    int32_t* ragged, int32_t* padded, int64_t maxlen, int pre_padding, int pre_truncating,
                    int32_t value, void* stream);
+
+/* ---- IMDB-C's corruptions (TextCorruptor.corrupt) ----------------------------------------------------------
+ * Texts are one strict UTF-8 byte buffer text[text_off[t] .. text_off[t+1]) per text (n_texts + 1 offsets,
+ * n_texts < 2^31).  Every output is string for string what the host port's corrupt() returns.  The arithmetic:
+ *   classes   cls[cp] for every code point present (TIP_CORRUPT_CP_WORDS * 32 entries): 0 whitespace (re's \s),
+ *             1 word (re's \w), 2 other.  A word is a maximal run of class 1, or of class 2, code points
+ *             (re.findall(r"\w+|[^\w\s]+", text)); words are numbered text-major, position-minor.
+ *   md5mod(m) int(md5(m).hexdigest(), 16) % 10**6: the digest as a big-endian 128-bit integer.
+ *   seeds     sentence seed S = md5mod(the text's words joined by single spaces) + seed (seed >= 0, S < 2^63);
+ *             word i's seed s_i = S + i.
+ *   rng(x)    NumPy's default_rng(x): SeedSequence(x).generate_state(4, uint64) = w0..w3 (x >= 2^32 enters as two
+ *             little-endian uint32 words), PCG64 with inc = (w2:w3) << 1 | 1, state = 0, one step, state += w0:w1,
+ *             one step; a step is state = state * 0x2360ED051FC65DA4_4385DF649FCCF645 + inc (mod 2^128); next64 =
+ *             one step, then (hi ^ lo) rotated right by state >> 122; random() = (next64 >> 11) * 2^-53; uint32
+ *             draws are buffered (one next64 gives its low half, then its high half).
+ *   types     rng(S): one random() u per word, type = the entries of type_cdf[4] <= u (searchsorted, side right),
+ *             type k being CorruptionType(k): 0 TYPO, 1 SYNONYM, 2 AUTOCOMPLETE, 3 AUTOCORRECT.
+ *   chosen    a second rng(S) shuffles 0..n-1 as Generator.shuffle: for i = n-1 .. 1, swap i with j =
+ *             random_interval(i) (mask = the smallest 2^b - 1 >= i, uint32 draws & mask until <= i); the first
+ *             rint(n * severity) (half to even, in double) shuffled indexes are chosen.
+ *   a chosen word w of >= 2 code points becomes, by its type (h = md5mod(w + " " + str(s_i))):
+ *     TYPO          code point k = s_i % len(w) replaced by letter h % L of a..z without w[k] (L = 25 when w[k] is
+ *                   in a..z, else 26);
+ *     AUTOCOMPLETE  the values of the bag keyed by w's first min(5, len) code points, then 4, then 3, without w
+ *                   itself: value h % (their number), in order; no such bag left: AUTOCORRECT;
+ *     AUTOCORRECT   w unchanged unless it is a common-word key; then value v0 + (the entries of val_cdf[v0 .. v1) <=
+ *                   rng(s_i).random()) of its range [v0, v1); an empty range sets *error_word = min(its word index)
+ *                   (the host port's Generator.choice raises there);
+ *     SYNONYM       the thesaurus value md5mod(w + " " + str(s_i) + " _corrupt_synonym") % (v1 - v0); no key or an
+ *                   empty range: TYPO.
+ *   output    each text's words (changed or not) joined by single spaces.
+ * A table maps distinct keys (arena[key_off[i] .. + key_len[i]), n < 2^31) to value ranges val_begin[i] ..
+ * val_begin[i+1] of strings arena[val_off[v] .. + val_len[v]); slots [cap] (cap a power of two >= 2 n) and key_hash
+ * [n] are filled by tip_corrupt_table_build.  Lookups compare hash, length and bytes, so a hash collision never
+ * changes a result.  val_cdf (common words only): Generator.choice's cdf of each key's candidates. */
+#define TIP_CORRUPT_CP_WORDS 34816 /* 0x110000 / 32 */
+typedef struct tip_corrupt_table {
+  const uint8_t* arena;
+  const int64_t* key_off;
+  const int32_t* key_len;
+  uint64_t* key_hash;
+  const int64_t* val_begin;    /* [n + 1] */
+  const int64_t* val_off;
+  const int32_t* val_len;
+  const double* val_cdf;       /* nullable except for the common-word table */
+  int32_t* slots;              /* [cap], -1 = empty */
+  int64_t n, cap;
+} tip_corrupt_table;
+/* tip_corrupt_table_build: key_hash and slots of a table (host struct, device arrays); n == 0 launches nothing.
+ * tip_corrupt_census: bitmap [TIP_CORRUPT_CP_WORDS] = bit cp set for every non-ASCII code point of text[0, n_bytes).
+ * tip_corrupt_count: n_words[t] = the words of text t.
+ * tip_corrupt_texts: word_off [n_texts + 1] = exclusive scan of n_words; per word: w_start (byte offset), w_len
+ *   (bytes), w_cps (code points), w_text, w_seed (s_i) and w_flags (type | 4 when chosen); perm [n_words] scratch.
+ *   type_cdf is a HOST array of 4 doubles.
+ * tip_corrupt_words: per word the result's source (o_src: 0 text, 1 common, 2 bags, 3 thesaurus arena), byte
+ *   offset in it and length, and o_typo = -1 or (byte offset of the replaced code point << 16 | its byte length << 8
+ *   | the letter); *error_word = 0x7f7f7f7f7f7f7f7f when no word failed.
+ * tip_corrupt_layout: o_pos = each word's output offset within its text, text_len[t] = its output bytes.
+ * tip_corrupt_write: out[out_off[t] + ...] = the output of text t (out_off: exclusive scan of text_len). */
+int tip_corrupt_table_build(const tip_corrupt_table* table, void* stream);
+int tip_corrupt_census(const uint8_t* text, int64_t n_bytes, uint32_t* bitmap, void* stream);
+int tip_corrupt_count(const uint8_t* text, const int64_t* text_off, int64_t n_texts, const uint8_t* cls,
+                      int64_t* n_words, void* stream);
+int tip_corrupt_texts(const uint8_t* text, const int64_t* text_off, int64_t n_texts, const uint8_t* cls,
+                      const int64_t* word_off, int64_t seed, double severity, const double* type_cdf, int64_t* w_start,
+                      int32_t* w_len, int32_t* w_cps, int32_t* w_text, int64_t* w_seed, uint8_t* w_flags, int32_t* perm,
+                      void* stream);
+int tip_corrupt_words(const uint8_t* text, const int64_t* w_start, const int32_t* w_len, const int32_t* w_cps,
+                      const int64_t* w_seed, const uint8_t* w_flags, int64_t n_words, const tip_corrupt_table* common,
+                      const tip_corrupt_table* bags, const tip_corrupt_table* thesaurus, uint8_t* o_src, int64_t* o_off,
+                      int32_t* o_len, int64_t* o_typo, int64_t* error_word, void* stream);
+int tip_corrupt_layout(const int64_t* word_off, int64_t n_texts, const int32_t* o_len, const int64_t* o_typo,
+                       int64_t* o_pos, int64_t* text_len, void* stream);
+int tip_corrupt_write(const uint8_t* text, const int32_t* w_text, const int64_t* word_off, int64_t n_words,
+                      const tip_corrupt_table* common, const tip_corrupt_table* bags,
+                      const tip_corrupt_table* thesaurus, const uint8_t* o_src, const int64_t* o_off,
+                      const int32_t* o_len, const int64_t* o_typo, const int64_t* o_pos, const int64_t* out_off,
+                      uint8_t* out, void* stream);
 
 /* ---- one training step of the case studies' models (case_study_*.py `model.fit`) -------------------------------
  * One parameter tensor of tip_keras_adam's table: param, its gradient and Adam's two moments, numel float32

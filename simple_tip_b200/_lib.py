@@ -45,6 +45,16 @@ class McLayer(C.Structure):
                 ("out", C.c_int32), ("activation", C.c_int32), ("reserved", C.c_int32)]
 
 
+class CorruptTable(C.Structure):
+    """tip_corrupt_table of include/b200tip.h"""
+    _fields_ = [("arena", C.c_void_p), ("key_off", C.c_void_p), ("key_len", C.c_void_p), ("key_hash", C.c_void_p),
+                ("val_begin", C.c_void_p), ("val_off", C.c_void_p), ("val_len", C.c_void_p), ("val_cdf", C.c_void_p),
+                ("slots", C.c_void_p), ("n", C.c_int64), ("cap", C.c_int64)]
+
+
+CORRUPT_CP_WORDS = 34816        # TIP_CORRUPT_CP_WORDS
+
+
 class WorkItem(C.Structure):
     _fields_ = [("q_row0", C.c_int32), ("q_rows", C.c_int32), ("col0", C.c_int32), ("col1", C.c_int32),
                 ("slot", C.c_int32), ("reserved", C.c_int32)]
@@ -131,6 +141,14 @@ _SIGNATURES = {
                               _i64, _vp, _i64, _vp, _vp]),
     "tip_tok_lookup": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _i64, _i64, _vp, _i64,
                                  _vp, _vp, _vp, _vp, _i64, C.c_int, C.c_int, _i32, _vp]),
+    "tip_corrupt_table_build": (C.c_int, [_vp, _vp]),
+    "tip_corrupt_census": (C.c_int, [_vp, _i64, _vp, _vp]),
+    "tip_corrupt_count": (C.c_int, [_vp, _vp, _i64, _vp, _vp, _vp]),
+    "tip_corrupt_texts": (C.c_int, [_vp, _vp, _i64, _vp, _vp, _i64, C.c_double, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                    _vp, _vp]),
+    "tip_corrupt_words": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "tip_corrupt_layout": (C.c_int, [_vp, _i64, _vp, _vp, _vp, _vp, _vp]),
+    "tip_corrupt_write": (C.c_int, [_vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "tip_keras_adam": (C.c_int, [_vp, _i32, _i64, _vp, _f32, _f32, _f32, _f32, _vp]),
     "tip_softmax_xent": (C.c_int, [_vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp]),
     "tip_softmax_xent_seg": (C.c_int, [_vp, _vp, _i64, _i64, _i32, _vp, _vp, _vp, _vp]),

@@ -12,6 +12,10 @@ Line references are to the reference's src/core/text_corruptor.py.  Where this m
   candidates: the same values, without the quadratic steps.
 SYNONYM corruptions pick from list(set(...)) of str (:435-444), whose order depends on PYTHONHASHSEED: like the
 reference's, they are reproducible only under a fixed hash seed.
+
+corrupt(..., backend="device") (or B200TIP_CORRUPT=device) runs the corruption loop on the GPU (csrc/corrupt.cu):
+the same strings, the same cache file.  It refuses seed < 0, and seeds where seed + 10**6 + the longest text's
+UTF-8 byte count reaches 2**63, with ValueError before any launch; the host path stays the default.
 """
 from __future__ import annotations
 
@@ -21,6 +25,7 @@ import enum
 import hashlib
 import json
 import logging
+import operator
 import os
 import pickle
 import re
@@ -132,6 +137,14 @@ def _generate_corruption_types(
     return [_TYPES[k] for k in idx]
 
 
+def _corrupt_backend(backend: Optional[str]) -> str:
+    """backend=None: the B200TIP_CORRUPT environment variable, default "host"."""
+    backend = backend if backend is not None else os.environ.get("B200TIP_CORRUPT", "host")
+    if backend not in ("host", "device"):
+        raise ValueError(f"backend must be 'host' or 'device', got {backend!r}")
+    return backend
+
+
 def _hash_text_to_int(words: List[str]) -> int:
     """:149-154"""
     return int(_hash_text_to_str(words), 16) % 1000000
@@ -178,6 +191,7 @@ class TextCorruptor(object):
         self.start_bags: Dict[int, Dict[str, List[str]]] = self._word_start_bags()
         self.lev_dist: np.ndarray = self._calculate_distances()
         self.thesaurus: Dict[str, List[str]] = self.load_bad_translations()
+        self._device_tables = None
 
     def _cache_file(self, name: str) -> Optional[str]:
         return None if self.cache_dir is None else os.path.join(self.cache_dir, name)
@@ -247,11 +261,14 @@ class TextCorruptor(object):
         seed: int,
         weights: Optional[CorruptionWeights] = None,
         force_recalculate: bool = False,
+        backend: Optional[str] = None,
     ) -> List[str]:
         """:311-410 — corrupts round(len(words) * severity) words of each text (words shorter than 2 characters
         stay), with per-text seeds from the text's md5, so that a text's corruption depends on neither the other
         texts nor their order, and a higher severity keeps the corruptions of a lower one.  Cached per
-        (texts, severity, seed) — not per weights — unless force_recalculate."""
+        (texts, severity, seed) — not per weights — unless force_recalculate.  backend: "host" (default) or
+        "device" (the GPU, string for string the same; None reads B200TIP_CORRUPT)."""
+        backend = _corrupt_backend(backend)
         assert 0 <= severity <= 1, "Severity must be between 0 and 1."
         cache_file = None
         if self.cache_dir is not None:
@@ -278,12 +295,86 @@ class TextCorruptor(object):
                     new_text.append(self._corrupt_word(word, sentence_seed + i, corruption_types[i]))
             return " ".join(new_text)
 
-        corrupted_texts = [_corrupt_single_text(text) for text in split_by_whitespace(texts)]
+        if backend == "device":
+            corrupted_texts, failed = self._corrupt_on_device(texts, severity, seed, weights)
+            if failed is not None:       # the host's exception for the first text that raises there
+                _corrupt_single_text(split_by_whitespace([texts[failed]])[0])
+                raise RuntimeError(f"the device reported text {failed} as failing, but the host corrupts it")
+        else:
+            corrupted_texts = [_corrupt_single_text(text) for text in split_by_whitespace(texts)]
         if cache_file is not None:
             os.makedirs(os.path.dirname(cache_file), exist_ok=True)
             with open(cache_file, "wb") as f:
                 pickle.dump(corrupted_texts, f)
         return corrupted_texts
+
+    def _corrupt_on_device(self, texts: List[str], severity: float, seed: int, weights: CorruptionWeights):
+        """(corrupted texts, None) from the device, or (None, t) when text t is the first for which the host path
+        raises (an unencodable text, invalid weights, an autocorrect without candidates)."""
+        from .. import engine as E
+
+        seed = operator.index(seed)
+        if isinstance(severity, bool) or not isinstance(severity, (int, float)):
+            raise TypeError(f"the device backend takes an int or float severity, got {type(severity).__name__}")
+        encoded, failed = [], None
+        for k, t in enumerate(texts):
+            try:
+                encoded.append(t.encode("utf-8"))
+            except UnicodeEncodeError:
+                failed = k
+                break
+        longest = max(map(len, encoded), default=0)
+        if seed < 0 or seed + 10 ** 6 + longest >= 2 ** 63:
+            raise ValueError(f"the device backend needs 0 <= seed and seed + 10**6 + {longest} (the longest text's "
+                             f"bytes) < 2**63, got seed={seed}")
+        w = np.array([weights.typo_weight, weights.autocomplete_weight, weights.autocorrect_weight,
+                      weights.synonym_weight])
+        normalized_weights = w / w.sum()
+        cdf = np.ones(4)                  # used only when no text has words
+        if np.any(normalized_weights < 0) or abs(normalized_weights.sum() - 1.0) > np.sqrt(np.finfo(np.float64).eps):
+            # _generate_corruption_types raises at the first text with words
+            first = next((k for k, t in enumerate(texts[:len(encoded)]) if split_by_whitespace([t])[0]), None)
+            if first is not None:
+                return None, first
+        else:
+            cdf = normalized_weights.cumsum()
+            cdf /= cdf[-1]
+        out, bad = E.corrupt_texts(encoded, self.device_tables(), seed, severity, cdf)
+        if bad is not None:
+            return None, bad
+        if failed is not None:
+            return None, failed
+        return [b.decode("utf-8", "surrogatepass") for b in out], None
+
+    def _autocorrect_choice(self, word_index: int):
+        """(np.argsort(lev_dist[k])[1:6], 1 / distance normalised) of common word k, computed once."""
+        cached = self._autocorrect_candidates.get(word_index)
+        if cached is None:
+            candidate_indices = np.argsort(self.lev_dist[word_index])[1:6]
+            candidate_distances = 1 / self.lev_dist[word_index][candidate_indices]
+            cached = (candidate_indices, candidate_distances / candidate_distances.sum())
+            self._autocorrect_candidates[word_index] = cached
+        return cached
+
+    def device_tables(self):
+        """The (common words, start bags, thesaurus) tables of the device backend, built on first use and kept."""
+        if getattr(self, "_device_tables", None) is None:
+            from .. import engine as E
+
+            values, cdfs = [], []
+            for k in range(len(self.common_words)):
+                candidate_indices, p = self._autocorrect_choice(k)
+                values.append([self.common_words[i] for i in candidate_indices])
+                if len(p):                # Generator.choice's cdf
+                    cdf = p.cumsum()
+                    cdf /= cdf[-1]
+                    cdfs.append(cdf)
+            common = E.CorruptTable(self.common_words, values, np.concatenate(cdfs) if cdfs else np.zeros(0))
+            bag_items = [item for n in sorted(self.start_bags) for item in self.start_bags[n].items()]
+            bags = E.CorruptTable([key for key, _ in bag_items], [bag for _, bag in bag_items])
+            thesaurus = E.CorruptTable(list(self.thesaurus), list(self.thesaurus.values()))
+            self._device_tables = (common, bags, thesaurus)
+        return self._device_tables
 
     def load_bad_translations(self) -> Dict[str, List[str]]:
         """:412-446 — {word: list(set(synonyms))} of the thesaurus lines with more than one synonym.  The thesaurus
@@ -341,13 +432,7 @@ class TextCorruptor(object):
         word_index = self._word_index.get(word)
         if word_index is None:
             return word
-        cached = self._autocorrect_candidates.get(word_index)
-        if cached is None:
-            candidate_indices = np.argsort(self.lev_dist[word_index])[1:6]
-            candidate_distances = 1 / self.lev_dist[word_index][candidate_indices]
-            cached = (candidate_indices, candidate_distances / candidate_distances.sum())
-            self._autocorrect_candidates[word_index] = cached
-        candidate_indices, p = cached
+        candidate_indices, p = self._autocorrect_choice(word_index)
         chosen_index = _get_rng(seed).choice(candidate_indices, p=p)
         return self.common_words[chosen_index]
 

@@ -20,6 +20,8 @@ from __future__ import annotations
 import ctypes as C
 import math
 import os
+import re
+import time
 from typing import Optional, Sequence, Tuple
 
 import numpy as np
@@ -2025,6 +2027,160 @@ def tok_lookup(words: TokWords, vocab: TokVocab, num_words: int, ragged: bool, m
                                           _p(padded), 0 if maxlen is None else maxlen, int(padding == "pre"),
                                           int(truncating == "pre"), value, _stream()), "tip_tok_lookup")
     return ids, kept_off, padded
+
+
+# ---- IMDB-C's corruptions (corrupt.cu) ---------------------------------------------------------------------------
+CORRUPT_CHUNK_BYTES = 1 << 28      # input bytes per chunk; every text is corrupted on its own, so chunking changes nothing
+_CP_CLASS = {}                     # code point -> 0 whitespace, 1 word, 2 other, as Python's re classifies it
+
+
+def _cp_class(cp: int) -> int:
+    c = _CP_CLASS.get(cp)
+    if c is None:
+        ch = chr(cp)
+        c = _CP_CLASS[cp] = 0 if re.match(r"\s", ch) else 1 if re.match(r"\w", ch) else 2
+    return c
+
+
+class CorruptTable:
+    """One word table of tip_corrupt_words on the device: distinct keys -> lists of strings (cdf: for the common
+    words, the flat float64 Generator.choice cdf of every list, in value order).  Strings are stored as UTF-8
+    ("surrogatepass"); a lookup compares bytes, so a hash collision never changes a result."""
+
+    def __init__(self, keys: Sequence[str], values: Sequence[Sequence[str]], cdf: Optional[np.ndarray] = None):
+        dev = require_cuda()
+        n = len(keys)
+        enc = [k.encode("utf-8", "surrogatepass") for k in keys]
+        enc += [v.encode("utf-8", "surrogatepass") for vals in values for v in vals]
+        lens = np.fromiter(map(len, enc), dtype=np.int64, count=len(enc))
+        if lens.size and int(lens.max()) >= 2 ** 31:
+            raise ValueError("a table string has 2^31 bytes or more")
+        off = np.zeros(len(enc), dtype=np.int64)
+        np.cumsum(lens[:-1], out=off[1:])
+        begin = np.zeros(n + 1, dtype=np.int64)
+        np.cumsum(np.fromiter(map(len, values), dtype=np.int64, count=n), out=begin[1:])
+
+        def up(a, dtype):
+            return torch.from_numpy(np.concatenate([np.asarray(a, dtype=dtype), np.zeros(1, dtype)])).to(dev)
+
+        self.n, self.cap = n, _pow2_at_least(2 * n)
+        self.arena = torch.from_numpy(np.frombuffer(bytearray(b"".join(enc)) + b"\0", dtype=np.uint8)).to(dev)
+        self.key_off, self.key_len = up(off[:n], np.int64), up(lens[:n], np.int32)
+        self.val_off, self.val_len = up(off[n:], np.int64), up(lens[n:], np.int32)
+        self.val_begin = up(begin, np.int64)
+        self.val_cdf = None if cdf is None else up(cdf, np.float64)
+        self.key_hash = torch.empty(n + 1, dtype=torch.int64, device=dev)
+        self.slots = torch.empty(self.cap, dtype=torch.int32, device=dev)
+        self.struct = _lib.CorruptTable(*(t.data_ptr() if t is not None else 0 for t in (
+            self.arena, self.key_off, self.key_len, self.key_hash, self.val_begin, self.val_off, self.val_len,
+            self.val_cdf, self.slots)), n, self.cap)
+        _lib.check(_lib.load().tip_corrupt_table_build(C.addressof(self.struct), _stream()), "tip_corrupt_table_build")
+
+
+def _class_table(bitmap: torch.Tensor) -> np.ndarray:
+    """uint8 [0x110000] classes of ASCII and of the non-ASCII code points the census found (others are never read)."""
+    bits = np.unpackbits(bitmap.cpu().numpy().view(np.uint8), bitorder="little")
+    cls = np.zeros(bits.size, dtype=np.uint8)
+    for cp in list(range(128)) + np.flatnonzero(bits).tolist():
+        cls[cp] = _cp_class(cp)
+    return cls
+
+
+def corrupt_texts(encoded: Sequence[bytes], tables: Sequence[CorruptTable], seed: int, severity: float,
+                  type_cdf: np.ndarray, chunk_bytes: int = CORRUPT_CHUNK_BYTES,
+                  timing: Optional[dict] = None) -> Tuple[list, Optional[int]]:
+    """tip_corrupt_* of the strict-UTF-8 texts `encoded` with the (common, bags, thesaurus) tables: (the corrupted
+    texts as UTF-8 bytes, None), or (the texts before it, t) when text t is the first with a chosen word whose
+    autocorrect has no candidates (the host port raises there).  Texts go in chunks of about chunk_bytes; the result
+    does not depend on the chunking.  timing, when given, accumulates "census_ms" (the census and the host's
+    classification) and "kernels_ms" (CUDA events around the other launches)."""
+    if seed < 0 or not 0.0 <= severity <= 1.0:
+        raise ValueError("seed must be >= 0 and severity in [0, 1]")
+    cdf = np.ascontiguousarray(type_cdf, dtype=np.float64)
+    if cdf.shape != (4,):
+        raise ValueError("type_cdf must have 4 entries")
+    out, t0 = [], 0
+    while t0 < len(encoded):
+        t1, size = t0 + 1, len(encoded[t0])
+        while t1 < len(encoded) and t1 - t0 < 2 ** 31 - 1 and size + len(encoded[t1]) <= chunk_bytes:
+            size += len(encoded[t1])
+            t1 += 1
+        texts, failed = _corrupt_chunk(encoded[t0:t1], tables, seed, float(severity), cdf, timing)
+        out += texts
+        if failed is not None:
+            return out, t0 + failed
+        t0 = t1
+    return out, None
+
+
+def _corrupt_chunk(encoded, tables, seed, severity, cdf, timing):
+    dev = require_cuda()
+    lib = _lib.load()
+    st = _stream()
+    n_t = len(encoded)
+    off = np.zeros(n_t + 1, dtype=np.int64)
+    np.cumsum(np.fromiter(map(len, encoded), dtype=np.int64, count=n_t), out=off[1:])
+    if int(np.max(np.diff(off))) >= 2 ** 31:
+        raise ValueError("a text has 2^31 bytes or more; word lengths are int32")
+    marks = []
+
+    def mark():
+        if timing is not None:
+            e = torch.cuda.Event(enable_timing=True)
+            e.record()
+            marks.append(e)
+
+    c0 = time.perf_counter()
+    text = torch.from_numpy(np.frombuffer(bytearray(b"".join(encoded)) + b"\0", dtype=np.uint8)).to(dev)
+    text_off = torch.from_numpy(off).to(dev)
+    bitmap = torch.empty(_lib.CORRUPT_CP_WORDS, dtype=torch.int32, device=dev)
+    _lib.check(lib.tip_corrupt_census(_p(text), int(off[-1]), _p(bitmap), st), "tip_corrupt_census")
+    cls = torch.from_numpy(_class_table(bitmap)).to(dev)
+    if timing is not None:
+        timing["census_ms"] = timing.get("census_ms", 0.0) + 1e3 * (time.perf_counter() - c0)
+    mark()
+    n_words = torch.empty(n_t, dtype=torch.int64, device=dev)
+    _lib.check(lib.tip_corrupt_count(_p(text), _p(text_off), n_t, _p(cls), _p(n_words), st), "tip_corrupt_count")
+    mark()
+    word_off = np.zeros(n_t + 1, dtype=np.int64)
+    np.cumsum(n_words.cpu().numpy(), out=word_off[1:])
+    nw = int(word_off[-1])
+    word_off_d = torch.from_numpy(word_off).to(dev)
+    mark()
+    w = max(nw, 1)
+    w_start, w_seed, o_off, o_typo, o_pos = torch.empty((5, w), dtype=torch.int64, device=dev)
+    w_len, w_cps, w_text, perm, o_len = torch.empty((5, w), dtype=torch.int32, device=dev)
+    w_flags, o_src = torch.empty((2, w), dtype=torch.uint8, device=dev)
+    err = torch.empty(1, dtype=torch.int64, device=dev)
+    _lib.check(lib.tip_corrupt_texts(_p(text), _p(text_off), n_t, _p(cls), _p(word_off_d), seed, severity,
+                                     cdf.ctypes.data, _p(w_start), _p(w_len), _p(w_cps), _p(w_text), _p(w_seed),
+                                     _p(w_flags), _p(perm), st), "tip_corrupt_texts")
+    common, bags, thesaurus = (C.addressof(t.struct) for t in tables)
+    _lib.check(lib.tip_corrupt_words(_p(text), _p(w_start), _p(w_len), _p(w_cps), _p(w_seed), _p(w_flags), nw, common,
+                                     bags, thesaurus, _p(o_src), _p(o_off), _p(o_len), _p(o_typo), _p(err), st),
+               "tip_corrupt_words")
+    text_len = torch.empty(n_t, dtype=torch.int64, device=dev)
+    _lib.check(lib.tip_corrupt_layout(_p(word_off_d), n_t, _p(o_len), _p(o_typo), _p(o_pos), _p(text_len), st),
+               "tip_corrupt_layout")
+    mark()
+    failed_word = int(err.item())
+    if failed_word < nw:
+        return [], int(np.searchsorted(word_off, failed_word, side="right")) - 1
+    out_off = np.zeros(n_t + 1, dtype=np.int64)
+    np.cumsum(text_len.cpu().numpy(), out=out_off[1:])
+    out_off_d = torch.from_numpy(out_off).to(dev)
+    mark()
+    out = torch.empty(max(int(out_off[-1]), 1), dtype=torch.uint8, device=dev)
+    _lib.check(lib.tip_corrupt_write(_p(text), _p(w_text), _p(word_off_d), nw, common, bags, thesaurus, _p(o_src),
+                                     _p(o_off), _p(o_len), _p(o_typo), _p(o_pos), _p(out_off_d), _p(out), st),
+               "tip_corrupt_write")
+    mark()
+    raw = out[:int(out_off[-1])].cpu().numpy().tobytes()
+    if timing is not None:
+        # kernel spans only: count, texts / words / layout, write (the gaps hold the host's scans)
+        timing["kernels_ms"] = timing.get("kernels_ms", 0.0) + sum(
+            marks[i].elapsed_time(marks[i + 1]) for i in (0, 2, 4))
+    return [raw[a:b] for a, b in zip(out_off[:-1].tolist(), out_off[1:].tolist())], None
 
 
 # ---- one training step of the case studies' models (train.cu) ----------------------------------------------------
