@@ -63,6 +63,7 @@
  *   tip_stack_gather    ... one step's batch for every model of a stack, in one launch
  *   tip_mc_head         handler_model.py get_pred_and_uncertainty: MC-dropout samples of a model's dropout head
  *                       (dropout masks, dense layers and softmax) from its trunk activations, in one launch
+ *   tip_mc_head_stack   the same for the M heads of a stack of models, one seed per model
  */
 #ifndef B200TIP_H
 #define B200TIP_H
@@ -783,6 +784,15 @@ typedef struct tip_mc_layer {
  * The draws depend on (seed, l, r, s, j) only: not on the launch shape, the row split or the sample split. */
 int tip_mc_head(const float* h, int64_t rows, int64_t ld, int64_t row0, int64_t sample0, int64_t samples,
                 const tip_mc_layer* layers, int32_t n_layers, uint64_t seed, int32_t mode, float* out, void* stream);
+/* tip_mc_head_stack: tip_mc_head on `models` heads of one shape (a stack's), in one launch per 256 models.
+ * layers[l].kernel is [models][in][out] and layers[l].bias [models][out]; model m's row i of h starts at
+ * h + m * ldm + i * ld (ldm = 0: every model reads the same rows); seeds [models] (host memory) = one seed per model;
+ * out [models][rows][samples][C].  out[m] is bit for bit what tip_mc_head writes for model m's h, kernels, biases
+ * and seeds[m] (same rows, row0, sample0, samples, rates, activations and mode): the key above with seed = seeds[m],
+ * so the model index enters through the seed only. */
+int tip_mc_head_stack(const float* h, int64_t models, int64_t rows, int64_t ld, int64_t ldm, int64_t row0,
+                      int64_t sample0, int64_t samples, const tip_mc_layer* layers, int32_t n_layers,
+                      const uint64_t* seeds, int32_t mode, float* out, void* stream);
 
 /* ---- bring-up / validation: plain accumulator dump ------------------------------------
  * out[256*256] (fp32, row-major, leading dimension 256) = tail-augmented dot products of q rows

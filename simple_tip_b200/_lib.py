@@ -154,6 +154,7 @@ _SIGNATURES = {
     "tip_softmax_xent_seg": (C.c_int, [_vp, _vp, _i64, _i64, _i32, _vp, _vp, _vp, _vp]),
     "tip_stack_gather": (C.c_int, [_vp, _i32, _i64, _vp, _i64, _vp, _i64, _i64, _i64, _i64, _i64, _vp, _vp]),
     "tip_mc_head": (C.c_int, [_vp, _i64, _i64, _i64, _i64, _i64, _vp, _i32, _u64, _i32, _vp, _vp]),
+    "tip_mc_head_stack": (C.c_int, [_vp, _i64, _i64, _i64, _i64, _i64, _i64, _i64, _vp, _i32, _vp, _i32, _vp, _vp]),
 }
 
 _lock = threading.Lock()

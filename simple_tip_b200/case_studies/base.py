@@ -11,7 +11,8 @@ the attention projections [embed, heads, key_dim] / [heads, key_dim, embed]), Co
 `CaseStudy` runs the reference's four phases for a torch model — `train`, `run_prio_eval`,
 `run_active_learning_eval`, `collect_activations` — over an output folder, one model after the other (uwiz's
 process pool and its `context` are not part of it).  `train` and `run_active_learning_eval` can instead train their
-models together in one stack (`stacked=True`, `core.training.fit_stack`), in one process on one GPU.
+models together in one stack (`stacked=True`, `core.training.fit_stack`), in one process on one GPU, and
+`run_prio_eval(stacked=True)` scores the fault predictors of a stack of models in one pass.
 """
 from __future__ import annotations
 
@@ -314,10 +315,26 @@ class CaseStudy:
             os.makedirs(os.path.dirname(path), exist_ok=True)
             torch.save(model.state_dict(), path)
 
-    def run_prio_eval(self, model_ids: Sequence[int]) -> Dict[int, dict]:
+    def run_prio_eval(self, model_ids: Sequence[int], stacked: bool = False,
+                      stack_size: Optional[int] = None) -> Dict[int, dict]:
         """`_prioritization_evaluator` per id: `core.prioritization.evaluate` with the case study's layers and
-        badge sizes; returns {model_id: its APFDs}."""
+        badge sizes; returns {model_id: its APFDs}.  stacked=True loads the ids' models and evaluates them in stacks
+        of at most `stack_size` (None: all ids in one) with `core.prioritization.evaluate_stack`, which writes the
+        same files and scores the fault predictors of a stack in one pass."""
         res = {}
+        if stacked:
+            if stack_size is not None and stack_size < 1:
+                raise ValueError(f"stack_size must be >= 1, got {stack_size}")
+            ids = list(model_ids)
+            size = stack_size or max(len(ids), 1)
+            for k in range(0, len(ids), size):
+                chunk = ids[k:k + size]
+                res.update(prioritization.evaluate_stack(
+                    chunk, self.name, [self.load_model(i) for i in chunk], self.train_set[0], self.nominal_set[0],
+                    self.nominal_set[1], self.ood_set[0], self.ood_set[1], self.nc_layers, self.sa_layers,
+                    dsa_badge_size=self.dsa_badge_size, output_folder=self.output_folder,
+                    batch_size=self.prediction_badge_size))
+            return res
         for model_id in model_ids:
             res[model_id] = prioritization.evaluate(
                 model_id, self.name, self.load_model(model_id), self.train_set[0], self.nominal_set[0],

@@ -148,12 +148,29 @@ def mc_head_layers(model) -> Tuple[int, List[HeadLayer]]:
     ends in a dense layer, and a softmax ends it.  Anything else raises ValueError naming the module.  (-1, []) when
     the model has no dropout module at all."""
     import torch
-    from torch.nn.modules.dropout import _DropoutNd
 
     from ..case_studies.base import Dense
 
     if not isinstance(model, torch.nn.Sequential):
         raise ValueError(f"sampler='head' needs a torch.nn.Sequential model, got {type(model).__name__}")
+    return _head_layers(model, Dense)
+
+
+def mc_head_layers_stack(stack) -> Tuple[int, List[HeadLayer]]:
+    """`mc_head_layers` for a `StackedSequential`: the same checks and messages, with `StackedDense` layers (kernel
+    [M, in, out], bias [M, out]) in the place of Dense."""
+    from ..case_studies.stacked import StackedDense, StackedSequential
+
+    if not isinstance(stack, StackedSequential):
+        raise ValueError(f"the stacked head sampler needs a StackedSequential, got {type(stack).__name__}")
+    return _head_layers(stack, StackedDense)
+
+
+def _head_layers(model, dense) -> Tuple[int, List[HeadLayer]]:
+    """mc_head_layers' parse of a Sequential whose dense layers are `dense` modules."""
+    import torch
+    from torch.nn.modules.dropout import _DropoutNd
+
     children = list(model.children())
     first = next((i for i, m in enumerate(children) if isinstance(m, _DropoutNd)), -1)
     if first < 0:
@@ -172,7 +189,7 @@ def mc_head_layers(model) -> Tuple[int, List[HeadLayer]]:
             if p is not None:
                 raise ValueError(f"sampler='head': {where} is a second dropout before one dense layer")
             p = float(m.p)
-        elif isinstance(m, Dense):
+        elif isinstance(m, dense):
             if m.activation not in (None, "relu", "softmax"):
                 raise ValueError(f"sampler='head': {where} has activation {m.activation!r}")
             layers.append(HeadLayer(p or 0.0, m, m.activation))
@@ -199,7 +216,7 @@ def mc_head_layers(model) -> Tuple[int, List[HeadLayer]]:
 
 def _head_tensors(layers: Sequence[HeadLayer], dev):
     """(kernel [in, out], bias [out], p, activation) per layer as contiguous float32 on dev; Linear weights are
-    transposed once."""
+    transposed once.  A stack's StackedDense layers give kernel [M, in, out] and bias [M, out]."""
     import torch
 
     out = []
@@ -372,6 +389,167 @@ def get_pred_and_uncertainty(model, x, batch_size: int = 32, sample_size: int = 
         for m, training in modes:
             m.training = training
     return pred, uncertainties, times
+
+
+
+def get_pred_and_uncertainty_stack(stack, x, batch_size: int = 32, sample_size: int = DROPOUT_SAMPLE_SIZE,
+                                   seeds: Optional[Sequence[int]] = None, sampler: Optional[str] = None
+                                   ) -> List[Tuple[np.ndarray, Dict[str, np.ndarray], Dict[str, List[float]]]]:
+    """`get_pred_and_uncertainty` for the M models of a `StackedSequential` (`case_studies.stacked.stack`) on the
+    same inputs x: one (pred, uncertainties, times) triple per model, in stack order, each in the form
+    `get_pred_and_uncertainty` returns.
+
+    The point pass is one stacked forward per batch of `batch_size` inputs (the batch repeated for every model in the
+    stack's input layout), and max softmax, PCS, softmax entropy and DeepGini each run once over the [M * N, C]
+    probabilities.  seeds: M ints, None = M zeros (each model's `seed` of `get_pred_and_uncertainty`).
+
+    sampler as in `get_pred_and_uncertainty`.  "head": the point pass captures the head's input [M, B, D] from the
+    stack (`mc_head_layers_stack`) and `tip_mc_head_stack` samples every model's head, model m's masks keyed by
+    seeds[m] exactly as `tip_mc_head` keys a single model's, in launches of MC_ROWS_PER_PASS model-rows; the votes
+    go to one `Votes` over the M * N rows.  "torch": the stack's own dropout modules in training mode, on batches
+    replicated up to MC_ROWS_PER_PASS model-rows per pass, drawing from torch's RNG seeded once with seeds[0]: every
+    model gets its own masks (dropout acts element-wise on the stacked tensor, as in `fit_stack`), which are not the
+    masks `get_pred_and_uncertainty` would draw for that model alone.
+
+    times: each phase is timed once for the whole stack and split evenly, so times[name] = [0, prediction time / M,
+    quantifier time / M, 0] (for "VR": sampling and vote time / M).  Every module's mode is restored afterwards.
+    ValueError, before any work, for a module that is not a StackedSequential, a seed count other than M, an
+    unknown sampler, a head the head sampler cannot sample, or an empty x."""
+    import torch
+    from torch.nn.modules.dropout import _DropoutNd
+
+    from . import quantifiers as Q
+    from .deepgini import DeepGini
+    from .timer import Timer
+    from .. import engine as E
+    from ..case_studies.stacked import StackedSequential
+
+    if not isinstance(stack, StackedSequential):
+        raise ValueError(f"get_pred_and_uncertainty_stack takes a StackedSequential, got {type(stack).__name__}")
+    n_models = len(stack.sources)
+    seeds = [0] * n_models if seeds is None else [int(s) for s in seeds]
+    if len(seeds) != n_models:
+        raise ValueError(f"{len(seeds)} seeds for a stack of {n_models} models")
+    sampler = sampler if sampler is not None else os.environ.get("B200TIP_MC", "torch")
+    if sampler not in MC_SAMPLERS:
+        raise ValueError(f"sampler must be one of {MC_SAMPLERS}, got {sampler!r}")
+    head_at, head = mc_head_layers_stack(stack) if sampler == "head" else (-1, [])
+    score_dev = E.require_cuda()
+    dev = next(iter(stack.parameters()), torch.empty(0)).device
+    if not isinstance(x, torch.Tensor):
+        x = torch.from_numpy(np.ascontiguousarray(x))
+    if x.shape[0] == 0:
+        raise ValueError("x holds no inputs")
+    x = x.to(dev)
+    n = x.shape[0]
+
+    def synced(fn, timer):
+        with timer:
+            res = fn()
+            torch.cuda.synchronize(score_dev)
+            if dev.type == "cuda" and dev != score_dev:
+                torch.cuda.synchronize(dev)
+        return res
+
+    def forward(xb):
+        return stack(stack.stack_inputs([xb] * n_models)).detach()
+
+    def point_pass():
+        outs = []
+        with torch.no_grad():
+            for start in range(0, n, batch_size):
+                outs.append(forward(x[start:start + batch_size]))
+        return torch.cat(outs, dim=1) if len(outs) != 1 else outs[0]
+
+    modes = [(m, m.training) for m in stack.modules()]
+    uncertainties: List[Dict[str, np.ndarray]] = [{} for _ in range(n_models)]
+    times: List[Dict[str, List[float]]] = [{} for _ in range(n_models)]
+    trunk: List[torch.Tensor] = []
+    hook = (list(stack.children())[head_at].register_forward_pre_hook(lambda _m, inp: trunk.append(inp[0].detach()))
+            if head else None)
+    try:
+        stack.eval()
+        pred_timer = Timer()
+        try:
+            probs = synced(point_pass, pred_timer)
+        finally:
+            if hook is not None:
+                hook.remove()
+        if probs.dim() != 3 or probs.shape[:2] != (n_models, n):
+            raise ValueError(f"the stack returned {tuple(probs.shape)}, expected [{n_models}, {n}, classes]")
+        c = probs.shape[2]
+        flat = probs.reshape(n_models * n, c)
+        pred = None
+        for q in (Q.MaxSoftmax, Q.PredictionConfidenceScore, Q.SoftmaxEntropy, DeepGini):
+            timer = Timer()
+            q_pred, values = synced(lambda: q.calculate(flat), timer)
+            if pred is None:
+                pred = q_pred.reshape(n_models, n)
+            name = q.aliases()[0].replace("custom::", "")
+            values = q.cast_conf_or_unc(False, values).reshape(n_models, n)
+            for m in range(n_models):
+                uncertainties[m][name] = values[m]
+                times[m][name] = [0, pred_timer.get() / n_models, timer.get() / n_models, 0]
+
+        dropouts = [m for m in stack.modules() if isinstance(m, _DropoutNd)]
+        votes = Q.Votes(n_models * n, c, score_dev) if head or dropouts else None
+        sampling_timer, vote_timer = Timer(), Timer()
+
+        def vote(out, samples, start, rows):
+            # out [M, rows, samples, C] (or its [M, rows * samples, C] view); model m's rows are votes rows m * n + i
+            for m in range(n_models):
+                votes.add(out[m], samples, sample_stride=c, row_stride=samples * c, row0=m * n + start, rows=rows)
+
+        if head:
+            for t in trunk:
+                if t.dim() != 3 or t.dtype != torch.float32 or t.shape[0] != n_models:
+                    raise ValueError(f"sampler='head' needs the head's input as 3-D float32 [{n_models}, B, D], got "
+                                     f"{tuple(t.shape)} {t.dtype}")
+            h = E.to_device(torch.cat(trunk, dim=1) if len(trunk) != 1 else trunk[0], score_dev)
+            if h.shape[1] != n:
+                raise ValueError(f"the head saw {h.shape[1]} rows, the stack's output has {n}")
+            layers = _head_tensors(head, score_dev)
+            rows_per_pass = max(1, MC_ROWS_PER_PASS // n_models)
+            for start in range(0, n if sample_size >= 1 else 0, rows_per_pass):
+                b = min(rows_per_pass, n - start)
+                out = synced(lambda: E.mc_head_stack(h[:, start:start + b], layers, seeds, sample_size, row0=start),
+                             sampling_timer)
+                if out.shape[3] != c:
+                    raise ValueError(f"the head gives {out.shape[3]} classes, the stack's output {c}")
+                synced(lambda: vote(out, sample_size, start, b), vote_timer)
+        elif dropouts:
+            for m in dropouts:
+                m.train()
+            with torch.random.fork_rng(devices=[dev] if dev.type == "cuda" else []), torch.no_grad():
+                torch.default_generator.manual_seed(seeds[0])
+                if dev.type == "cuda":
+                    with torch.cuda.device(dev):
+                        torch.cuda.manual_seed(seeds[0])
+                for start in range(0, n, batch_size):
+                    xb = x[start:start + batch_size]
+                    b = xb.shape[0]
+                    done = 0
+                    while done < sample_size:
+                        r = min(sample_size - done, max(1, MC_ROWS_PER_PASS // (b * n_models)))
+                        # row i * r + j of a model's pass is replica j of input i: [b, r, C] once viewed
+                        xr = xb.unsqueeze(1).expand(b, r, *xb.shape[1:]).reshape(b * r, *xb.shape[1:])
+                        out = synced(lambda: forward(xr), sampling_timer)
+                        if tuple(out.shape) != (n_models, b * r, c):
+                            raise ValueError(f"an MC-dropout pass returned {tuple(out.shape)}, expected "
+                                             f"{(n_models, b * r, c)}")
+                        o = out if out.dtype in (torch.float32, torch.float64) else out.to(torch.float32)
+                        synced(lambda: vote(E.to_device(o, score_dev), r, start, b), vote_timer)
+                        done += r
+        if head or dropouts:
+            _, vr = synced(lambda: votes.finish(sample_size), vote_timer)
+            vr = vr.reshape(n_models, n)
+            for m in range(n_models):
+                uncertainties[m]["VR"] = vr[m]
+                times[m]["VR"] = [0, sampling_timer.get() / n_models, vote_timer.get() / n_models, 0]
+    finally:
+        for m, training in modes:
+            m.training = training
+    return [(pred[m], uncertainties[m], times[m]) for m in range(n_models)]
 
 
 def _badge_dir(root: str, case_study: str, model_id: int, dataset: str) -> str:

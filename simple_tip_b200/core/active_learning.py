@@ -59,8 +59,10 @@ def evaluate(model_id: int, case_study: str, model, train_x, train_y, nominal_te
     observed split, concatenated once on the inputs' device (a torch tensor), y_pool their labels the same way (one-hot
     as above, on x_pool's device), and rows the int64 [selections, n] tensor of pool rows on that device whose row k
     is exactly the retraining set `training_process` would receive for selection k (`np.random.permutation` is drawn
-    once per selection, in the same order).  It returns the retrained models in selection order, which are then
-    evaluated one by one as the sequential loop evaluates them.
+    once per selection, in the same order).  It returns the retrained models in selection order.  When they are
+    `KerasSequential` networks of one architecture (a case study's `stacked_training_process`), they are evaluated
+    together, one stacked forward per badge and split (`accuracies_stack`); other modules are evaluated one by one
+    as the sequential loop evaluates them.
 
     Returns (original model's accuracies, selections, {(metric, "nominal" / "ood"): retrained model's accuracies}),
     each dict in the reference's insertion order; the reference returns None."""
@@ -85,9 +87,9 @@ def evaluate(model_id: int, case_study: str, model, train_x, train_y, nominal_te
     if stacked_training_process is not None:
         new_models = _retrain_stacked(num_classes, stacked_training_process, train_x, train_y, active_datasets,
                                       selections)
-        for key, new_model in zip(selections, new_models):
-            active_accuracies[key] = _evaluate(new_model, active_datasets, num_classes, batch_size)
-        del new_models, new_model
+        for key, eval_res in zip(selections, _evaluate_stack(new_models, active_datasets, num_classes, batch_size)):
+            active_accuracies[key] = eval_res
+        del new_models
     else:
         for (metric, ood_or_nom), selected_indexes in selections.items():
             x, y = active_datasets[ood_or_nom, OBS]
@@ -296,6 +298,54 @@ def accuracy(model, x, y, batch_size: int = 128) -> float:
         for m, training in modes:
             m.training = training
     return int(correct.item()) / n
+
+
+def accuracies_stack(stack, x, y, batch_size: int = 128) -> list:
+    """`accuracy` of each of the M models of a `StackedSequential` (`case_studies.stacked.stack`) on the same (x, y),
+    from one stacked forward per batch of `batch_size`: model m's exact correct / n, its correct count summed from the
+    first-index argmax of its slice [b, classes] of the stacked softmax output.  The stack runs in eval mode without
+    gradients; its modes are restored afterwards."""
+    import torch
+
+    m = len(stack.sources)
+    dev = next(iter(stack.parameters()), torch.empty(0)).device
+    labels = _as_tensor(y, dev).reshape(-1)
+    n = labels.shape[0]
+    modes = [(module, module.training) for module in stack.modules()]
+    correct = torch.zeros(m, dtype=torch.int64, device=dev)
+    stack.eval()
+    try:
+        with torch.no_grad():
+            for start in range(0, n, batch_size):
+                xb = _as_tensor(x[start:start + batch_size], dev)
+                out = stack(stack.stack_inputs([xb] * m))                # [M, b, classes]
+                correct += (out.argmax(dim=2) == labels[start:start + batch_size]).sum(dim=1)
+    finally:
+        for module, training in modes:
+            module.training = training
+    return [int(c) / n for c in correct.tolist()]
+
+
+def _evaluate_stack(models: Sequence, datasets: SplitDataset, num_classes: Optional[int], batch_size: int = 128
+                    ) -> list:
+    """`_evaluate` of every model, one SplitEvaluation per model in order.  `KerasSequential` networks of one
+    architecture (what a case study's `stacked_training_process` returns) are scored together, one stacked forward
+    per batch and split (`accuracies_stack`); any other modules one by one with `_evaluate`."""
+    from ..case_studies.base import KerasSequential
+    from ..case_studies.stacked import stack
+
+    if not models or not all(isinstance(m, KerasSequential) for m in models):
+        return [_evaluate(m, datasets, num_classes, batch_size) for m in models]
+    net = stack(models)
+    res = [dict() for _ in models]
+    for (ood_or_nom, observed_or_future), (x, y) in datasets.items():
+        for eval_res, acc in zip(res, accuracies_stack(net, x, y, batch_size)):
+            assert 0 <= acc <= 1, (
+                "The models metric is not accuracy, change your "
+                "training_process callable."
+            )
+            eval_res[ood_or_nom, observed_or_future] = acc
+    return res
 
 
 def _evaluate(model, datasets: SplitDataset, num_classes: Optional[int], batch_size: int = 128) -> SplitEvaluation:

@@ -78,6 +78,67 @@ def evaluate(model_id: int, case_study: str, model, training_dataset, nominal_te
     return res
 
 
+def evaluate_stack(model_ids: Sequence[int], case_study: str, models: Sequence, training_dataset,
+                   nominal_test_dataset, nominal_test_labels, ood_test_dataset, ood_test_labels,
+                   nc_activation_layers: Sequence, sa_activation_layers: Sequence,
+                   dsa_badge_size: Optional[int] = None, output_folder: str = OUTPUT_FOLDER, batch_size: int = 128
+                   ) -> Dict[int, Dict[str, Dict[str, float]]]:
+    """`evaluate` for M models of one architecture (`KerasSequential` networks, model k has id model_ids[k]):
+    every file `evaluate(model_ids[k], ..., models[k], ...)` writes, under the same names.
+
+    The fault predictors of both datasets come from one `case_studies.stacked.stack(models)`
+    (`activations.get_pred_and_uncertainty_stack`, its defaults as `evaluate` takes the single-model ones); the
+    coverage and the surprise arm then run model by model, in `evaluate`'s order, each arm freed before the next.
+    Their score and CAM-order files are those of `evaluate`; the fault predictors' are those of the stacked forward,
+    which equals each model's own forward to rounding (the torch sampler's masks differ: see
+    `get_pred_and_uncertainty_stack`), and their time files hold each phase's time split evenly over the M models.
+
+    Returns {model_id: what `evaluate` returns for it}.  ValueError, before any forward pass, for the conditions
+    `evaluate` refuses, for len(models) != len(model_ids) and for repeated model ids."""
+    from ..case_studies.stacked import stack
+
+    model_ids = [int(i) for i in model_ids]
+    if len(model_ids) != len(models):
+        raise ValueError(f"{len(model_ids)} model ids for {len(models)} models")
+    if len(set(model_ids)) != len(model_ids):
+        raise ValueError(f"model ids {model_ids} repeat")
+    if "_" in case_study:
+        raise ValueError(f"case_study {case_study!r} contains '_', which the result file names cannot carry")
+    labels = {NOM: _flat_labels(nominal_test_labels, nominal_test_dataset, "nominal_test_labels"),
+              OOD: _flat_labels(ood_test_labels, ood_test_dataset, "ood_test_labels")}
+    datasets = {NOM: nominal_test_dataset, OOD: ood_test_dataset}
+
+    masks: Dict[int, Dict[str, np.ndarray]] = {i: {} for i in model_ids}
+    scores: Dict[int, Dict[str, Arrays]] = {i: {NOM: {}, OOD: {}} for i in model_ids}
+    cam_orders: Dict[int, Dict[str, Arrays]] = {i: {NOM: {}, OOD: {}} for i in model_ids}
+    stacked = stack(models)
+    for ds in (NOM, OOD):
+        per_model = activations.get_pred_and_uncertainty_stack(stacked, datasets[ds])
+        for model_id, (pred, uncertainties, times) in zip(model_ids, per_model):
+            masks[model_id][ds], scores[model_id][ds] = _persist_fault_predictors(
+                output_folder, case_study, model_id, labels[ds], ds, pred, uncertainties, times)
+    del stacked, per_model
+    gc.collect()
+
+    res: Dict[int, Dict[str, Dict[str, float]]] = {}
+    for model_id, model in zip(model_ids, models):
+        nc_scores, nc_orders = _eval_neuron_coverage(output_folder, case_study, model, model_id, datasets,
+                                                     training_dataset, nc_activation_layers, batch_size)
+        gc.collect()
+        sa_scores, sa_orders = _eval_surprise(output_folder, case_study, model, model_id, datasets, training_dataset,
+                                              sa_activation_layers, batch_size, dsa_badge_size)
+        gc.collect()
+        res[model_id] = {}
+        for ds in (NOM, OOD):
+            scores[model_id][ds].update(nc_scores[ds])
+            scores[model_id][ds].update(sa_scores[ds])
+            cam_orders[model_id][ds].update(nc_orders[ds])
+            cam_orders[model_id][ds].update(sa_orders[ds])
+            apfds = results.apfd_values(masks[model_id][ds], scores[model_id][ds], cam_orders[model_id][ds])
+            res[model_id][ds] = {approach: apfds[approach] for approach in results.APPROACHES if approach in apfds}
+    return res
+
+
 def _host(a) -> np.ndarray:
     try:
         import torch
@@ -101,6 +162,11 @@ def _flat_labels(labels, data, what: str) -> np.ndarray:
 def _eval_fault_predictors(output_folder, case_study, model, model_id, x, labels, ds) -> Tuple[np.ndarray, Arrays]:
     """eval_prioritization.py:193-215: the misclassification mask, every quantifier's uncertainties and times."""
     pred, uncertainties, times = activations.get_pred_and_uncertainty(model, x)
+    return _persist_fault_predictors(output_folder, case_study, model_id, labels, ds, pred, uncertainties, times)
+
+
+def _persist_fault_predictors(output_folder, case_study, model_id, labels, ds, pred, uncertainties, times
+                              ) -> Tuple[np.ndarray, Arrays]:
     is_misclassified = pred != labels
     results.persist(output_folder, case_study, ds, "is_misclassified", model_id, is_misclassified)
     for metric, t in times.items():

@@ -13,7 +13,13 @@
 //
 // Heads with more than one layer (TW > 0: SPT = 1, WP = TW) keep layer 0's activations in registers x[TW] and run
 // the later layers (widths <= TW <= 64) from shared memory, fully unrolled, with the same masks and order.
+//
+// tip_mc_head_stack runs M heads of one shape (a StackedSequential's) in one launch: blockIdx.y picks the model, whose
+// h, kernels, biases, output and seed the block uses; the pair space, the tiling and the key are tip_mc_head's, so
+// model m's slice is bit for bit tip_mc_head's launch on model m.  tip_mc_head is the body with model 0.
 #include <math.h>
+
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -43,6 +49,14 @@ struct McArgs {
   float* out;
   int n_layers, mode;
   McLayer L[kMcMaxLayers];
+};
+
+constexpr int kMcStackChunk = 256;  // models per tip_mc_head_stack launch: their seeds ride in the kernel parameters
+
+struct McStackArgs : McArgs {      // kernels [M][in][out], biases [M][out], out [M][rows][samples][C]
+  int64_t ldm;                      // h: model m's row i at h + m * ldm + i * ld
+  int64_t model0;                   // the launch's first model
+  uint64_t seeds[kMcStackChunk];    // seeds[blockIdx.y] = model model0 + blockIdx.y's
 };
 
 __device__ __forceinline__ uint64_t mc_key(uint64_t seed, int layer, int64_t row, int64_t sample) {
@@ -83,8 +97,27 @@ __device__ __forceinline__ void mc_store(float (&z)[N], int C, int act, int mode
     if (c < C) dst[c] = __fdiv_rn(z[c], s);
 }
 
-template <int WP, int SPT, int TW>
-__global__ void __launch_bounds__(kMcThreads, 1) mc_head_kernel(const __grid_constant__ McArgs a) {
+// p + off for a stack's model; tip_mc_head's kernel (STACK = false) addresses a's pointers as they are
+template <bool STACK, class T>
+__device__ __forceinline__ T* mc_at(T* p, int64_t off) {
+  if constexpr (STACK) return p + off;
+  else return p;
+}
+
+// STACK = false: tip_mc_head's kernel on McArgs.  STACK = true: tip_mc_head_stack's on McStackArgs, block
+// (blockIdx.x, blockIdx.y) = tip_mc_head's block blockIdx.x on model model0 + blockIdx.y.
+template <int WP, int SPT, int TW, bool STACK = false>
+__global__ void __launch_bounds__(kMcThreads, 1)
+    mc_head_kernel(const __grid_constant__ std::conditional_t<STACK, McStackArgs, McArgs> p) {
+  const McArgs& a = p;
+  int64_t m = 0, ldm = 0;
+  const uint64_t* seedp = &a.seed;
+  if constexpr (STACK) {
+    m = p.model0 + blockIdx.y;
+    ldm = p.ldm;
+    seedp = &p.seeds[blockIdx.y];
+  }
+  const uint64_t& seed = *seedp;
   extern __shared__ __align__(16) float smem[];
   float* sK = smem;                                  // [kMcChunk][WP]
   float* sH = sK + kMcChunk * WP;                    // [kMcTileRows][kMcHStride]
@@ -105,7 +138,9 @@ __global__ void __launch_bounds__(kMcThreads, 1) mc_head_kernel(const __grid_con
       for (int i = tid; i < (in2 + 1) * TW; i += kMcThreads) {
         const int j = i / TW, c = i - j * TW;
         float v = 0.f;
-        if (c < L.out) v = j < L.in ? L.kernel[(int64_t)j * L.out + c] : (j == in2 ? L.bias[c] : 0.f);
+        if (c < L.out)
+          v = j < L.in ? mc_at<STACK>(L.kernel, m * L.in * L.out)[(int64_t)j * L.out + c]
+                       : (j == in2 ? mc_at<STACK>(L.bias, m * L.out)[c] : 0.f);
         w[i] = v;
       }
     }
@@ -118,7 +153,7 @@ __global__ void __launch_bounds__(kMcThreads, 1) mc_head_kernel(const __grid_con
     const int64_t q = min(q0 + tid + (int64_t)k * kMcThreads, q1 - 1);
     const int64_t r = q / S;
     rl[k] = (int)(r - r_lo) * kMcHStride;
-    key[k] = mc_key(a.seed, 0, a.row0 + r, a.sample0 + (q - r * S));
+    key[k] = mc_key(seed, 0, a.row0 + r, a.sample0 + (q - r * S));
   }
   float acc[SPT][WP];
 #pragma unroll
@@ -134,11 +169,11 @@ __global__ void __launch_bounds__(kMcThreads, 1) mc_head_kernel(const __grid_con
     __syncthreads();
     for (int i = tid; i < kMcChunk * WP; i += kMcThreads) {
       const int j = i / WP, c = i - j * WP;
-      sK[i] = (j < dn && c < W0) ? __ldg(L0.kernel + (int64_t)(d0 + j) * W0 + c) : 0.f;
+      sK[i] = (j < dn && c < W0) ? __ldg(mc_at<STACK>(L0.kernel, m * D * W0) + (int64_t)(d0 + j) * W0 + c) : 0.f;
     }
     for (int i = tid; i < n_rows * kMcChunk; i += kMcThreads) {
       const int r = i / kMcChunk, j = i - r * kMcChunk;
-      sH[r * kMcHStride + j] = j < dn ? __ldg(a.h + (r_lo + r) * a.ld + d0 + j) : 0.f;
+      sH[r * kMcHStride + j] = j < dn ? __ldg(mc_at<STACK>(a.h, m * ldm) + (r_lo + r) * a.ld + d0 + j) : 0.f;
     }
     __syncthreads();
     const int dn2 = (dn + 1) & ~1;
@@ -173,9 +208,9 @@ __global__ void __launch_bounds__(kMcThreads, 1) mc_head_kernel(const __grid_con
     if (q >= q1) break;
     float z[WP];
 #pragma unroll
-    for (int c = 0; c < WP; c++) z[c] = c < W0 ? __fadd_rn(acc[k][c], __ldg(L0.bias + c)) : 0.f;
+    for (int c = 0; c < WP; c++) z[c] = c < W0 ? __fadd_rn(acc[k][c], __ldg(mc_at<STACK>(L0.bias, m * W0) + c)) : 0.f;
     if constexpr (TW == 0) {
-      mc_store(z, W0, L0.act, a.mode, a.out + q * W0);
+      mc_store(z, W0, L0.act, a.mode, mc_at<STACK>(a.out, m * total * W0) + q * W0);
     } else {
       const int64_t r = q / S, s = q - r * S;
       float x[TW];
@@ -184,7 +219,7 @@ __global__ void __launch_bounds__(kMcThreads, 1) mc_head_kernel(const __grid_con
       for (int l = 1; l < a.n_layers; l++) {
         const McLayer& L = a.L[l];
         const float* w = sT + L.woff;
-        const uint64_t kl = mc_key(a.seed, l, a.row0 + r, a.sample0 + s);
+        const uint64_t kl = mc_key(seed, l, a.row0 + r, a.sample0 + s);
         float y[TW];
 #pragma unroll
         for (int c = 0; c < TW; c++) y[c] = 0.f;
@@ -209,7 +244,7 @@ __global__ void __launch_bounds__(kMcThreads, 1) mc_head_kernel(const __grid_con
 #pragma unroll
         for (int c = 0; c < TW; c++) y[c] = c < L.out ? __fadd_rn(y[c], bias[c]) : 0.f;
         if (l + 1 == a.n_layers) {
-          mc_store(y, L.out, L.act, a.mode, a.out + q * L.out);
+          mc_store(y, L.out, L.act, a.mode, mc_at<STACK>(a.out, m * total * L.out) + q * L.out);
         } else {
 #pragma unroll
           for (int c = 0; c < TW; c++) x[c] = c < L.out ? mc_act(y[c], L.act) : 0.f;
@@ -219,8 +254,9 @@ __global__ void __launch_bounds__(kMcThreads, 1) mc_head_kernel(const __grid_con
   }
 }
 
+// models == 0: tip_mc_head's launch of a; else models heads in launches of kMcStackChunk models, s's McArgs = a
 template <int WP, int SPT, int TW>
-int mc_launch(McArgs& a, cudaStream_t stream) {
+int mc_launch(McArgs& a, McStackArgs* s, int64_t models, const uint64_t* seeds, cudaStream_t stream) {
   a.pairs_per_block = min((int64_t)kMcThreads * SPT, (int64_t)(kMcTileRows - 1) * a.samples);
   const int64_t total = a.rows * a.samples;
   const int64_t grid = (total + a.pairs_per_block - 1) / a.pairs_per_block;
@@ -231,25 +267,34 @@ int mc_launch(McArgs& a, cudaStream_t stream) {
     tail += (((a.L[l].in + 1) & ~1) + 1) * TW;
   }
   const size_t bytes = sizeof(float) * ((size_t)kMcChunk * WP + (size_t)kMcTileRows * kMcHStride + tail);
-  auto kern = mc_head_kernel<WP, SPT, TW>;
+  if (models == 0) {
+    auto kern = mc_head_kernel<WP, SPT, TW>;
+    if (bytes > 48 * 1024) TIP_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    kern<<<(unsigned)grid, kMcThreads, bytes, stream>>>(a);
+    TIP_LAUNCH_CHECK();
+    return TIP_OK;
+  }
+  auto kern = mc_head_kernel<WP, SPT, TW, true>;
   if (bytes > 48 * 1024) TIP_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-  kern<<<(unsigned)grid, kMcThreads, bytes, stream>>>(a);
-  TIP_LAUNCH_CHECK();
+  static_cast<McArgs&>(*s) = a;
+  for (int64_t m0 = 0; m0 < models; m0 += kMcStackChunk) {
+    const int n = (int)min((int64_t)kMcStackChunk, models - m0);
+    s->model0 = m0;
+    for (int k = 0; k < n; k++) s->seeds[k] = seeds[m0 + k];
+    kern<<<dim3((unsigned)grid, (unsigned)n), kMcThreads, bytes, stream>>>(*s);
+    TIP_LAUNCH_CHECK();
+  }
   return TIP_OK;
 }
 
-}  // namespace tip
-
-extern "C" int tip_mc_head(const float* h, int64_t rows, int64_t ld, int64_t row0, int64_t sample0, int64_t samples,
-                           const tip_mc_layer* layers, int32_t n_layers, uint64_t seed, int32_t mode, float* out,
-                           void* stream) {
-  using namespace tip;
+// the layer table's checks and McArgs (everything but h, ld and out) of tip_mc_head and tip_mc_head_stack
+int mc_args(int64_t rows, int64_t row0, int64_t sample0, int64_t samples, const tip_mc_layer* layers,
+            int32_t n_layers, int32_t mode, McArgs& a, int& widest) {
   TIP_REQUIRE(layers && n_layers >= 1 && n_layers <= kMcMaxLayers, "1..4 layers");
   TIP_REQUIRE(mode == TIP_MC_OUTPUT || mode == TIP_MC_PREACT, "mode is TIP_MC_OUTPUT or TIP_MC_PREACT");
   TIP_REQUIRE(rows >= 0 && samples >= 1 && row0 >= 0 && sample0 >= 0, "rows >= 0, samples >= 1, row0, sample0 >= 0");
-  McArgs a;
   memset(&a, 0, sizeof(a));
-  int widest = 0;
+  widest = 0;
   for (int l = 0; l < n_layers; l++) {
     const tip_mc_layer& L = layers[l];
     TIP_REQUIRE(L.kernel && L.bias, "null kernel or bias");
@@ -270,30 +315,68 @@ extern "C" int tip_mc_head(const float* h, int64_t rows, int64_t ld, int64_t row
     d.act = L.activation;
     if (L.out > widest) widest = L.out;
   }
+  a.rows = rows;
+  a.row0 = row0;
+  a.sample0 = sample0;
+  a.samples = samples;
+  a.n_layers = n_layers;
+  a.mode = mode;
+  return TIP_OK;
+}
+
+int mc_dispatch(McArgs& a, int widest, McStackArgs* s, int64_t models, const uint64_t* seeds, cudaStream_t st) {
+  if (a.n_layers > 1) {
+    if (widest <= 8) return mc_launch<8, 1, 8>(a, s, models, seeds, st);
+    if (widest <= 16) return mc_launch<16, 1, 16>(a, s, models, seeds, st);
+    if (widest <= 32) return mc_launch<32, 1, 32>(a, s, models, seeds, st);
+    return mc_launch<64, 1, 64>(a, s, models, seeds, st);
+  }
+  if (widest <= 4) return mc_launch<4, 8, 0>(a, s, models, seeds, st);
+  if (widest <= 8) return mc_launch<8, 8, 0>(a, s, models, seeds, st);
+  if (widest <= 12) return mc_launch<12, 4, 0>(a, s, models, seeds, st);
+  if (widest <= 16) return mc_launch<16, 4, 0>(a, s, models, seeds, st);
+  if (widest <= 32) return mc_launch<32, 2, 0>(a, s, models, seeds, st);
+  return mc_launch<64, 1, 0>(a, s, models, seeds, st);
+}
+
+}  // namespace tip
+
+extern "C" int tip_mc_head(const float* h, int64_t rows, int64_t ld, int64_t row0, int64_t sample0, int64_t samples,
+                           const tip_mc_layer* layers, int32_t n_layers, uint64_t seed, int32_t mode, float* out,
+                           void* stream) {
+  using namespace tip;
+  McArgs a;
+  int widest = 0;
+  const int rc = mc_args(rows, row0, sample0, samples, layers, n_layers, mode, a, widest);
+  if (rc != TIP_OK) return rc;
   TIP_REQUIRE(out && (h || rows == 0), "null pointer");
   TIP_REQUIRE(ld >= layers[0].in, "row stride below the input width");
   if (rows == 0) return TIP_OK;
   a.h = h;
-  a.rows = rows;
   a.ld = ld;
-  a.row0 = row0;
-  a.sample0 = sample0;
-  a.samples = samples;
   a.seed = seed;
   a.out = out;
-  a.n_layers = n_layers;
-  a.mode = mode;
-  cudaStream_t s = (cudaStream_t)stream;
-  if (n_layers > 1) {
-    if (widest <= 8) return mc_launch<8, 1, 8>(a, s);
-    if (widest <= 16) return mc_launch<16, 1, 16>(a, s);
-    if (widest <= 32) return mc_launch<32, 1, 32>(a, s);
-    return mc_launch<64, 1, 64>(a, s);
-  }
-  if (widest <= 4) return mc_launch<4, 8, 0>(a, s);
-  if (widest <= 8) return mc_launch<8, 8, 0>(a, s);
-  if (widest <= 12) return mc_launch<12, 4, 0>(a, s);
-  if (widest <= 16) return mc_launch<16, 4, 0>(a, s);
-  if (widest <= 32) return mc_launch<32, 2, 0>(a, s);
-  return mc_launch<64, 1, 0>(a, s);
+  return mc_dispatch(a, widest, nullptr, 0, nullptr, (cudaStream_t)stream);
+}
+
+extern "C" int tip_mc_head_stack(const float* h, int64_t models, int64_t rows, int64_t ld, int64_t ldm, int64_t row0,
+                                 int64_t sample0, int64_t samples, const tip_mc_layer* layers, int32_t n_layers,
+                                 const uint64_t* seeds, int32_t mode, float* out, void* stream) {
+  using namespace tip;
+  McArgs a;
+  int widest = 0;
+  const int rc = mc_args(rows, row0, sample0, samples, layers, n_layers, mode, a, widest);
+  if (rc != TIP_OK) return rc;
+  TIP_REQUIRE(models >= 0 && ldm >= 0, "models >= 0, ldm >= 0");
+  TIP_REQUIRE(seeds || models == 0, "null seeds");
+  TIP_REQUIRE(out && (h || rows == 0 || models == 0), "null pointer");
+  TIP_REQUIRE(ld >= layers[0].in, "row stride below the input width");
+  if (rows == 0 || models == 0) return TIP_OK;
+  a.h = h;
+  a.ld = ld;
+  a.out = out;
+  McStackArgs s;
+  memset(&s, 0, sizeof(s));
+  s.ldm = ldm;
+  return mc_dispatch(a, widest, &s, models, seeds, (cudaStream_t)stream);
 }

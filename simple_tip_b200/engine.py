@@ -2311,6 +2311,35 @@ MC_MAX_WIDTH = 64         # units of every head layer
 MC_ACTIVATIONS = {None: _lib.MC_LINEAR, "linear": _lib.MC_LINEAR, "relu": _lib.MC_RELU, "softmax": _lib.MC_SOFTMAX}
 
 
+def _mc_table(layers, width: int, dev, models: Optional[int] = None):
+    """(tip_mc_layer table, the last layer's width) of engine.mc_head's `layers` on `width` inputs; models = M: each
+    kernel [M, in, out] and bias [M, out] (mc_head_stack).  ValueError for anything else."""
+    if not 1 <= len(layers) <= MC_MAX_LAYERS:
+        raise ValueError(f"an MC-dropout head has 1..{MC_MAX_LAYERS} dense layers, got {len(layers)}")
+    if not 1 <= width <= MC_MAX_IN:
+        raise ValueError(f"the head's input width must be 1..{MC_MAX_IN}, got {width}")
+    lead = () if models is None else (models,)
+    table = (_lib.McLayer * len(layers))()
+    for i, (kernel, bias, p, act) in enumerate(layers):
+        if act not in MC_ACTIVATIONS or (act == "softmax" and i != len(layers) - 1):
+            raise ValueError(f"layer {i}: activation {act!r} (linear, relu, or softmax on the last layer)")
+        for name, t, dim in (("kernel", kernel, 2 + len(lead)), ("bias", bias, 1 + len(lead))):
+            if (not isinstance(t, torch.Tensor) or t.dim() != dim or t.dtype != torch.float32 or t.device != dev
+                    or not t.is_contiguous()):
+                raise ValueError(f"layer {i}: {name} must be a contiguous {dim}-D float32 tensor on {dev}")
+        out = kernel.shape[-1]
+        if (tuple(kernel.shape[:-1]) != (*lead, width) or not 1 <= out <= MC_MAX_WIDTH
+                or tuple(bias.shape) != (*lead, out)):
+            raise ValueError(f"layer {i}: kernel {tuple(kernel.shape)} / bias {tuple(bias.shape)} do not take {width} "
+                             f"inputs to 1..{MC_MAX_WIDTH} units" + (f" for {models} models" if lead else ""))
+        p = float(p)
+        if not 0.0 <= p <= 1.0:
+            raise ValueError(f"layer {i}: dropout rate {p} outside [0, 1]")
+        table[i] = _lib.McLayer(kernel.data_ptr(), bias.data_ptr(), p, width, out, MC_ACTIVATIONS[act], 0)
+        width = out
+    return table, width
+
+
 def mc_head(h: torch.Tensor, layers, seed: int, samples: int, row0: int = 0, sample0: int = 0,
             out: Optional[torch.Tensor] = None, preact: bool = False) -> torch.Tensor:
     """tip_mc_head: `samples` MC-dropout samples of a dense head for every row of the trunk activations h
@@ -2331,25 +2360,7 @@ def mc_head(h: torch.Tensor, layers, seed: int, samples: int, row0: int = 0, sam
         raise ValueError(f"an MC-dropout head has 1..{MC_MAX_LAYERS} dense layers, got {len(layers)}")
     if samples < 1 or row0 < 0 or sample0 < 0:
         raise ValueError(f"samples >= 1, row0 >= 0 and sample0 >= 0, got {samples}, {row0}, {sample0}")
-    table = (_lib.McLayer * len(layers))()
-    width = h.shape[1]
-    if not 1 <= width <= MC_MAX_IN:
-        raise ValueError(f"the head's input width must be 1..{MC_MAX_IN}, got {width}")
-    for i, (kernel, bias, p, act) in enumerate(layers):
-        if act not in MC_ACTIVATIONS or (act == "softmax" and i != len(layers) - 1):
-            raise ValueError(f"layer {i}: activation {act!r} (linear, relu, or softmax on the last layer)")
-        for name, t, dim in (("kernel", kernel, 2), ("bias", bias, 1)):
-            if (not isinstance(t, torch.Tensor) or t.dim() != dim or t.dtype != torch.float32 or t.device != dev
-                    or not t.is_contiguous()):
-                raise ValueError(f"layer {i}: {name} must be a contiguous {dim}-D float32 tensor on {dev}")
-        if kernel.shape[0] != width or not 1 <= kernel.shape[1] <= MC_MAX_WIDTH or tuple(bias.shape) != (kernel.shape[1],):
-            raise ValueError(f"layer {i}: kernel {tuple(kernel.shape)} / bias {tuple(bias.shape)} do not take {width} "
-                             f"inputs to 1..{MC_MAX_WIDTH} units")
-        p = float(p)
-        if not 0.0 <= p <= 1.0:
-            raise ValueError(f"layer {i}: dropout rate {p} outside [0, 1]")
-        table[i] = _lib.McLayer(kernel.data_ptr(), bias.data_ptr(), p, width, kernel.shape[1], MC_ACTIVATIONS[act], 0)
-        width = kernel.shape[1]
+    table, width = _mc_table(layers, h.shape[1], dev)
     rows = h.shape[0]
     shape = (rows, samples, width)
     if out is None:
@@ -2360,4 +2371,41 @@ def mc_head(h: torch.Tensor, layers, seed: int, samples: int, row0: int = 0, sam
     _lib.check(_lib.load().tip_mc_head(_p(h), rows, ld, row0, sample0, samples, table, len(layers),
                                        int(seed) & 0xFFFFFFFFFFFFFFFF, _lib.MC_PREACT if preact else _lib.MC_OUTPUT,
                                        _p(out), _stream()), "tip_mc_head")
+    return out
+
+
+def mc_head_stack(h: torch.Tensor, layers, seeds, samples: int, row0: int = 0, sample0: int = 0,
+                  out: Optional[torch.Tensor] = None, preact: bool = False) -> torch.Tensor:
+    """tip_mc_head_stack: `mc_head` for the M heads of one shape of a stack, in one launch per 256 models.  h
+    [M, rows, D] (float32 on the current CUDA device, unit column stride, any row and model stride: a model stride
+    of 0, as `expand` gives, feeds every model the same rows); layers: 1..4 tuples (kernel [M, in, out], bias [M,
+    out], p, activation) as `mc_head` takes them with a leading model axis; seeds: M ints.  Returns out [M, rows,
+    samples, C] float32, whose slice m is bit for bit `mc_head(h[m], model m's layers, seeds[m], ...)`.  Raises
+    ValueError before any launch for anything else."""
+    dev = require_cuda()
+    if not isinstance(h, torch.Tensor) or h.dim() != 3 or h.dtype != torch.float32 or h.device != dev:
+        raise ValueError(f"h must be a 3-D float32 tensor [M, rows, D] on {dev}, got "
+                         f"{tuple(h.shape) if isinstance(h, torch.Tensor) else type(h).__name__}")
+    models, rows, d = h.shape
+    if models * rows > 0 and d > 1 and h.stride(2) != 1:
+        raise ValueError("h must have a unit column stride")
+    if min(h.stride()) < 0:
+        raise ValueError("h must have non-negative strides")
+    seeds = [int(s) for s in seeds]
+    if len(seeds) != models:
+        raise ValueError(f"{len(seeds)} seeds for {models} models")
+    if samples < 1 or row0 < 0 or sample0 < 0:
+        raise ValueError(f"samples >= 1, row0 >= 0 and sample0 >= 0, got {samples}, {row0}, {sample0}")
+    table, width = _mc_table(layers, d, dev, models)
+    shape = (models, rows, samples, width)
+    if out is None:
+        out = torch.empty(shape, dtype=torch.float32, device=dev)
+    elif tuple(out.shape) != shape or out.dtype != torch.float32 or out.device != dev or not out.is_contiguous():
+        raise ValueError(f"out must be a contiguous float32 {shape} tensor on {dev}")
+    ld = h.stride(1) if rows > 1 else d
+    ldm = h.stride(0) if models > 1 else 0
+    seed_table = (C.c_uint64 * max(models, 1))(*[s & 0xFFFFFFFFFFFFFFFF for s in seeds])
+    _lib.check(_lib.load().tip_mc_head_stack(_p(h), models, rows, ld, ldm, row0, sample0, samples, table, len(layers),
+                                             seed_table, _lib.MC_PREACT if preact else _lib.MC_OUTPUT, _p(out),
+                                             _stream()), "tip_mc_head_stack")
     return out
