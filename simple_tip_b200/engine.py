@@ -2219,6 +2219,15 @@ def keras_adam(table: torch.Tensor, n_tensors: int, total_numel: int, state: tor
                "tip_keras_adam")
 
 
+def _check_xent_outputs(z, y, loss, dz, correct, m: int) -> None:
+    """ValueError unless loss (float32) and correct (int32) hold m elements and every tensor is on z's CUDA device
+    (the kernel reads and writes them all through raw pointers)."""
+    if loss.numel() < m or correct.numel() < m or loss.dtype != torch.float32 or correct.dtype != torch.int32:
+        raise ValueError(f"loss (float32) and correct (int32) need {m} elements")
+    if not z.is_cuda or any(t is not None and t.device != z.device for t in (y, loss, dz, correct)):
+        raise ValueError(f"z, y, loss, dz and correct must be on one CUDA device, got z on {z.device}")
+
+
 def softmax_xent(z: torch.Tensor, y: torch.Tensor, loss: torch.Tensor, dz: Optional[torch.Tensor],
                  correct: torch.Tensor) -> None:
     """tip_softmax_xent into preallocated device outputs: loss (float32, 1 element) = the batch mean of the softmax
@@ -2228,6 +2237,7 @@ def softmax_xent(z: torch.Tensor, y: torch.Tensor, loss: torch.Tensor, dz: Optio
         raise ValueError(f"z and y must be float32 [B, C] of one shape, got {tuple(z.shape)}, {tuple(y.shape)}")
     if not (z.is_contiguous() and y.is_contiguous()) or (dz is not None and (dz.shape != z.shape or not dz.is_contiguous())):
         raise ValueError("z, y and dz must be contiguous")
+    _check_xent_outputs(z, y, loss, dz, correct, 1)
     lib = _lib.load()
     _lib.check(lib.tip_softmax_xent(_p(z), _p(y), z.shape[0], z.shape[1], _p(loss), _p(dz), _p(correct), _stream()),
                "tip_softmax_xent")
@@ -2243,8 +2253,7 @@ def softmax_xent_seg(z: torch.Tensor, y: torch.Tensor, loss: torch.Tensor, dz: O
     if not (z.is_contiguous() and y.is_contiguous()) or (dz is not None and (dz.shape != z.shape or not dz.is_contiguous())):
         raise ValueError("z, y and dz must be contiguous")
     m = z.shape[0]
-    if loss.numel() < m or correct.numel() < m or loss.dtype != torch.float32 or correct.dtype != torch.int32:
-        raise ValueError(f"loss (float32) and correct (int32) need {m} elements")
+    _check_xent_outputs(z, y, loss, dz, correct, m)
     lib = _lib.load()
     _lib.check(lib.tip_softmax_xent_seg(_p(z), _p(y), m, z.shape[1], z.shape[2], _p(loss), _p(dz), _p(correct),
                                         _stream()), "tip_softmax_xent_seg")
@@ -2274,11 +2283,17 @@ def stack_gather(pool: torch.Tensor, rows: torch.Tensor, perm: torch.Tensor, sta
     pool [N, ...] float32, float64 (gathered as float32) or int32 on the device; any other dtype is refused.
     interleaved=False: out [M, b, *row_shape] (model-major); True: a pool of NHWC rows [N, H, W, C] gives out
     [b, H, W, M * C], channel m * C + c of it being model m's channel c.  check=True checks the rows table against
-    the pool (`check_stack_rows`, a device-to-host read); a caller that already did passes False."""
+    the pool (`check_stack_rows`, a device-to-host read) and perm against [0, n) (one more); a caller that already
+    did passes False, and the values are then not checked."""
     if pool.dtype not in _GATHER_DTYPES:
         raise ValueError(f"tip_stack_gather gathers float32, float64 or int32 pools, not {pool.dtype}")
     if not pool.is_cuda or not pool.is_contiguous() or pool.dim() < 2:
         raise ValueError("pool must be a contiguous CUDA tensor [N, ...]")
+    if rows.device != pool.device or perm.device != pool.device:
+        raise ValueError(f"rows and perm must be on the pool's device {pool.device}, got {rows.device} and "
+                         f"{perm.device}")
+    if rows.dim() != 2 or rows.dtype != torch.int64 or not rows.is_contiguous():
+        raise ValueError(f"rows must be a contiguous int64 [M, n] tensor, got {tuple(rows.shape)} {rows.dtype}")
     if check:
         check_stack_rows(rows, pool.shape[0])
     if perm.dim() != 2 or perm.dtype != torch.int64 or not perm.is_contiguous() or perm.shape[0] != rows.shape[0]:
@@ -2287,6 +2302,10 @@ def stack_gather(pool: torch.Tensor, rows: torch.Tensor, perm: torch.Tensor, sta
     n_perm = perm.shape[1]
     if not (0 <= start and b >= 1 and start + b <= n_perm <= n_rows):
         raise ValueError(f"batch [{start}, {start + b}) outside a permutation of {n_perm} of {n_rows} rows")
+    if check:
+        lo, hi = torch.stack(torch.aminmax(perm)).tolist()
+        if lo < 0 or hi >= n_rows:
+            raise ValueError(f"perm index [{lo}, {hi}] outside each model's {n_rows} rows")
     dtype, out_dtype = _GATHER_DTYPES[pool.dtype]
     row_shape = tuple(pool.shape[1:])
     if interleaved:

@@ -3,24 +3,13 @@ replayed from a captured graph; tip_softmax_xent against a float64 NumPy referen
 import numpy as np
 import pytest
 
+from oracle.train_oracle import adam_restatement
+
 pytestmark = pytest.mark.gpu
 
 SIZES = (1, 3, 5, 1023, 4097, 1_600_000)
 STEPS = 20
 F = np.float32
-
-
-def _adam_reference(p, g_steps, lr=F(1e-3), b1=F(0.9), b2=F(0.999), eps=F(1e-7)):
-    """include/b200tip.h's order: every operation in float32, rounded once; beta^t in float64, rounded once."""
-    m, v = np.zeros_like(p), np.zeros_like(p)
-    one = F(1)
-    for t, g in enumerate(g_steps, start=1):
-        b1t, b2t = F(np.float64(b1) ** t), F(np.float64(b2) ** t)
-        lr_t = F(lr * F(F(np.sqrt(F(one - b2t))) / F(one - b1t)))
-        m = F(b1 * m) + F(F(one - b1) * g)
-        v = F(b2 * v) + F(F(one - b2) * F(g * g))
-        p = p - F(lr_t * m) / F(np.sqrt(v) + eps)
-    return p, m, v
 
 
 def _tables(torch, E, rng):
@@ -47,7 +36,7 @@ def _tables(torch, E, rng):
 
 def _check(views, p0, grads):
     for i in range(len(SIZES)):
-        p, m, v = _adam_reference(p0[i], [g[i] for g in grads])
+        p, m, v = adam_restatement(p0[i], [g[i] for g in grads])
         assert np.array_equal(views["p"][i].cpu().numpy(), p), f"param of tensor {i} ({SIZES[i]} elements)"
         assert np.array_equal(views["m"][i].cpu().numpy(), m), f"m of tensor {i}"
         assert np.array_equal(views["v"][i].cpu().numpy(), v), f"v of tensor {i}"
