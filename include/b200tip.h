@@ -306,6 +306,19 @@ int tip_nn_filter(const void* q_pack, const float* q_sqnorm, int64_t m, const vo
                   int32_t* cand_cnt, int32_t cap, int32_t n_static, int32_t* sched_counter,
                   void* stream);
 
+/* tip_nn_filter whose queries end per class at a bound known only on the device (DSA's stage 2 on distinct
+ * winners, tip_dsa_distinct_winners): q_live_end[m] (may be NULL: tip_nn_filter) holds, for every query row, one
+ * past the last row that holds a query in its class's range.  An item covers rows [q_row0, min(q_row0 + q_rows,
+ * q_live_end[q_row0])) of its tile; an item without such rows is skipped when it is drawn (no query-tile load, no
+ * pipeline stage), so a work list that draws its items through sched_counter (n_static == 0), ordered so that the
+ * rows likeliest to be live come first, keeps the CTAs balanced whatever the live counts turn out to be. */
+int tip_nn_filter_live(const void* q_pack, const float* q_sqnorm, int64_t m, const void* t_pack,
+                       int64_t n, int64_t d, int64_t pitch, const tip_work_item* items,
+                       int32_t n_items, const int32_t* q_class, const int32_t* class_off, float t_rmax,
+                       const float* q_rounderr, float t_errmax, uint32_t* row_min_bits, int32_t* cand_idx,
+                       int32_t* cand_cnt, int32_t cap, int32_t n_static, int32_t* sched_counter,
+                       const int32_t* q_live_end, void* stream);
+
 /* Tile geometry tip_nn_filter uses for traces of width d: work items must start on query rows
  * that are multiples of nothing in particular but cover at most *q_rows rows (192 for the resident-query
  * kernel, 128 for the streaming one); *t_rows is the train-tile height (128), useful for sizing spans. */
@@ -369,6 +382,31 @@ int tip_nn_rerank(const void* q, const void* t, int dtype, int64_t m, int64_t n,
                   void* next_pack, float* next_sqnorm, float* next_rounderr,
                   uint32_t* next_row_min_bits, int32_t* next_cand_cnt, const tip_rerank_extras* extras,
                   void* stream);
+
+/* DSA's stage 2 once per distinct stage-1 winner (its result depends on the winning train row alone,
+ * surprise.py:622-631).  pos[m]: stage-1 winner positions (tip_nn_rerank's out_pos) of class-sorted inputs whose
+ * class ranges are q_off[C+1] (device); class_off[C+1] (device) as for tip_nn_rerank, every class at most
+ * max_class_rows rows (tip_dsa_distinct_smem_bytes(max_class_rows) <= 48 KB).  Class c's slots are
+ * [q_off[c], q_off[c] + k[c]): its distinct winners in ascending train-row order, then one slot for its inputs without
+ * a winner (pos outside the class: a zero row is searched, as tip_nn_rerank's next_* packs it) if it has any.  For
+ * every slot s below the bound: rows[s] = the winner's train row (dtype, m x d), the packed stage-2 query state
+ * (what tip_nn_rerank's next_* with next_seed_ub = seed_ub writes for that row) and slot_class[s] = c; past it
+ * slot_class[s] = -1 (tip_nn_rerank writes "no row" there), cand_cnt[s] = 0 and the rest of the state is not
+ * written.  live_end[s] = q_off[c] +
+ * k[c] for every slot of class c (tip_nn_filter_live), slot[i] = the slot of input i.  blocks_per_class blocks share
+ * each class's slots.  Nothing is kept between calls. */
+int64_t tip_dsa_distinct_smem_bytes(int64_t max_class_rows);
+int tip_dsa_distinct_winners(const int32_t* pos, int64_t m, const int32_t* q_off, const int32_t* class_off,
+                             int32_t n_classes, int64_t max_class_rows, int32_t blocks_per_class, const void* t,
+                             int dtype, int64_t d, const float* center, const float* seed_ub, float t_rmax,
+                             float t_errmax, void* rows, void* q_pack, float* q_sqnorm, float* q_rounderr,
+                             uint32_t* row_min_bits, int32_t* cand_cnt, int32_t* slot_class, int32_t* live_end,
+                             int32_t* k, int32_t* slot, void* stream);
+/* dist_b[i] = slot_dist[slot[i]] for i < m; with out != NULL also the result scatter of tip_dsa_pack_out
+ * (dist_a, that dist_b, gid, dist_a / dist_b into column idx[i] of out[4 x n_total]). */
+int tip_dsa_slot_out(const void* slot_dist, int dtype, const int32_t* slot, int64_t m, const void* dist_a,
+                     const int32_t* gid, const int32_t* idx, int64_t n_total, void* dist_b, double* out,
+                     void* stream);
 
 /* DSA result packing (surprise.py:576-611 scatter by index): for i < m,
  *   out[0*n_total + j] = dist_a[i], out[1*n_total + j] = dist_b[i], out[2*n_total + j] = gid[i],

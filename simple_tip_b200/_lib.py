@@ -86,12 +86,18 @@ _SIGNATURES = {
     "tip_pair_prep": (C.c_int, [_vp, C.c_int, _i64, _i64, _vp, C.c_int, C.c_int, _f32, _f32, _vp, _vp, _vp, _vp]),
     "tip_nn_filter": (C.c_int, [_vp, _vp, _i64, _vp, _i64, _i64, _i64, _vp, _i32, _vp, _vp, _f32, _vp, _f32, _vp, _vp,
                                 _vp, _i32, _i32, _vp, _vp]),
+    "tip_nn_filter_live": (C.c_int, [_vp, _vp, _i64, _vp, _i64, _i64, _i64, _vp, _i32, _vp, _vp, _f32, _vp, _f32, _vp,
+                                     _vp, _vp, _i32, _i32, _vp, _vp, _vp]),
     "tip_sizeof_rerank_extras": (_i32, []),
     "tip_nn_rerank_work_bytes": (_i64, [_i64, C.c_int]),
     "tip_nn_query_prep": (C.c_int, [_vp, C.c_int, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "tip_nn_rerank": (C.c_int, [_vp, _vp, C.c_int, _i64, _i64, _i64, _vp, _vp, _i32, _vp, _vp, _i32, C.c_int,
                                 _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "tip_gather_rows": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp]),
+    "tip_dsa_distinct_smem_bytes": (_i64, [_i64]),
+    "tip_dsa_distinct_winners": (C.c_int, [_vp, _i64, _vp, _vp, _i32, _i64, _i32, _vp, C.c_int, _i64, _vp, _vp, _f32,
+                                           _f32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "tip_dsa_slot_out": (C.c_int, [_vp, C.c_int, _vp, _i64, _vp, _vp, _vp, _i64, _vp, _vp, _vp]),
     "tip_dsa_pack_out": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp, _i64, _i64, _vp, _vp]),
     "tip_comm_bytes": (_i64, [_i32, _i64]),
     "tip_comm_alloc": (C.c_int, [_i32, _i64, C.POINTER(C.c_void_p), _vp]),

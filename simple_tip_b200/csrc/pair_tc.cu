@@ -101,6 +101,9 @@ struct PairArgs {
   // form a pool that CTAs drain through the atomic counter once they run dry
   int n_static;
   int* sched_counter;
+  // optional (tip_nn_filter_live): query rows at and past q_live_end[q_row0] hold no query; an item's rows end there,
+  // and an item without rows is skipped by the producer (no query-tile load, no ring stage)
+  const int32_t* q_live_end;
   int k16;  // number of K=16 MMA steps per tile (packed width / 16)
   int64_t m;
   // MODE_NN
@@ -468,20 +471,24 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         long long n_tiles_done = 0, n_items_done = 0;
         int w_static = blockIdx.x;
         for (int k = 0;; k++) {
-          int w;
-          if (w_static < args.n_static) { w = w_static; w_static += gridDim.x; }
-          else if (args.sched_counter) {
-            w = args.n_static + atomicAdd(args.sched_counter, 1);
-            if (w >= args.n_items) w = -1;
-          } else w = -1;
+          int w, ntiles = 0;
+          tip_work_item it;
+          for (;;) {   // the next item with work: padding entries and items without live rows never reach the ring
+            if (w_static < args.n_static) { w = w_static; w_static += gridDim.x; }
+            else if (args.sched_counter) {
+              w = args.n_static + atomicAdd(args.sched_counter, 1);
+              if (w >= args.n_items) w = -1;
+            } else w = -1;
+            if (w < 0) break;
+            it = args.items[w];
+            ntiles = (it.col1 - it.col0 + BN - 1) / BN;
+            if (ntiles > 0 && (!args.q_live_end || args.q_live_end[it.q_row0] > it.q_row0)) break;
+          }
           const int slot = k & 1;
           mbar_wait(sched_empty(slot), ((uint32_t)(k >> 1) & 1u) ^ 1u);
           sched_ring[slot] = w;
           mbar_arrive(sched_full(slot));
           if (w < 0) break;
-          const tip_work_item it = args.items[w];
-          const int ntiles = (it.col1 - it.col0 + BN - 1) / BN;
-          if (ntiles <= 0) continue;   // padding entry of a balanced work list
           n_tiles_done += ntiles; n_items_done++;
           if (RESA && it.q_row0 != a_row0) {
             // the consumers arrive once they start an item of another query tile, when every MMA on this one has
@@ -601,9 +608,9 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         }
         break;
       }
-      const tip_work_item it = args.items[w];
+      tip_work_item it = args.items[w];
       const int ntiles = (it.col1 - it.col0 + BN - 1) / BN;
-      if (ntiles <= 0) continue;
+      if (args.q_live_end) it.q_rows = min(it.q_rows, args.q_live_end[it.q_row0] - it.q_row0);
       // a warpgroup whose 64 rows all lie past the item's query rows issues no MMAs; with no valid row its epilogue
       // only hands empty mailbox entries to the drain, and it keeps its place in the ring and query-tile protocols
       const bool idle = L::kWgs == 3 && __shfl_sync(0xffffffffu, (int)(64 * g >= it.q_rows), 0);
@@ -1106,12 +1113,12 @@ extern "C" int tip_debug_cta_clock(long long* buf) {
   return TIP_OK;
 }
 
-extern "C" int tip_nn_filter(const void* q_pack, const float* q_sqnorm, int64_t m, const void* t_pack, int64_t n,
-                             int64_t d, int64_t pitch, const tip_work_item* items, int32_t n_items,
-                             const int32_t* q_class, const int32_t* class_off, float t_rmax,
-                             const float* q_rounderr, float t_errmax, uint32_t* row_min_bits, int32_t* cand_idx,
-                             int32_t* cand_cnt, int32_t cap, int32_t n_static, int32_t* sched_counter,
-                             void* stream) {
+extern "C" int tip_nn_filter_live(const void* q_pack, const float* q_sqnorm, int64_t m, const void* t_pack, int64_t n,
+                                  int64_t d, int64_t pitch, const tip_work_item* items, int32_t n_items,
+                                  const int32_t* q_class, const int32_t* class_off, float t_rmax,
+                                  const float* q_rounderr, float t_errmax, uint32_t* row_min_bits, int32_t* cand_idx,
+                                  int32_t* cand_cnt, int32_t cap, int32_t n_static, int32_t* sched_counter,
+                                  const int32_t* q_live_end, void* stream) {
   TIP_REQUIRE(q_pack && q_sqnorm && t_pack && items && row_min_bits && cand_idx && cand_cnt, "null pointer");
   TIP_REQUIRE(cap >= 1 && n_items >= 0, "cap / n_items");
   TIP_REQUIRE(pitch == tip_pair_pitch(d, 1), "pitch does not match tip_pair_pitch(d, 1)");
@@ -1133,10 +1140,22 @@ extern "C" int tip_nn_filter(const void* q_pack, const float* q_sqnorm, int64_t 
   a.row_min_bits = row_min_bits; a.cand_idx = cand_idx; a.cand_cnt = cand_cnt; a.cap = cap;
   a.timeline = g_timeline; a.timeline_tiles = g_timeline_tiles;
   a.cta_clock = g_cta_clock;
+  a.q_live_end = q_live_end;
   const bool excl = q_class != nullptr && class_off != nullptr;   // per-query own-class masking compiled in only then
   const bool resa = a.k16 <= kRsMaxK16;
   return excl ? launch_pair<MODE_NN, true>(q_pack, m, t_pack, n, pitch, a, resa, (cudaStream_t)stream)
               : launch_pair<MODE_NN, false>(q_pack, m, t_pack, n, pitch, a, resa, (cudaStream_t)stream);
+}
+
+extern "C" int tip_nn_filter(const void* q_pack, const float* q_sqnorm, int64_t m, const void* t_pack, int64_t n,
+                             int64_t d, int64_t pitch, const tip_work_item* items, int32_t n_items,
+                             const int32_t* q_class, const int32_t* class_off, float t_rmax,
+                             const float* q_rounderr, float t_errmax, uint32_t* row_min_bits, int32_t* cand_idx,
+                             int32_t* cand_cnt, int32_t cap, int32_t n_static, int32_t* sched_counter,
+                             void* stream) {
+  return tip_nn_filter_live(q_pack, q_sqnorm, m, t_pack, n, d, pitch, items, n_items, q_class, class_off, t_rmax,
+                            q_rounderr, t_errmax, row_min_bits, cand_idx, cand_cnt, cap, n_static, sched_counter,
+                            nullptr, stream);
 }
 
 extern "C" int tip_nn_filter_tile(int64_t d, int32_t* q_rows, int32_t* t_rows) {

@@ -382,6 +382,139 @@ static int launch_rerank(const RerankArgs<T>& a, cudaStream_t st) {
   return TIP_OK;
 }
 
+// ---- DSA stage 2 on distinct winners ----------------------------------------------------------------
+// Stage 2 searches from stage 1's winning TRAIN row, so its result is a function of that row alone
+// (surprise.py:622-631): inputs that share a winner share a stage-2 search.  Block (c, p) of the compaction
+// rebuilds class c's winner set in shared memory — one bit per train row of the class, set from the stage-1
+// positions of the class's inputs — ranks the set bits by a prefix of word popcounts, and then does its 1/P share
+// of the class's slot range [q_off[c], q_off[c] + k_c): the packed stage-2 query state of every distinct winner, in
+// training-row order (deterministic, whatever order stage 1 finished in), the live bound and class of every slot,
+// and every input's slot.  Inputs without a winner (pos < 0: the filter and re-rank search from a zero row, as
+// write_result packs it) share one more slot after the winners.  Nothing persists between calls.
+constexpr int kCompactThreads = 256;
+
+template <typename T>
+struct CompactArgs {
+  const int32_t* pos;        // [m] stage-1 winner position per class-sorted input
+  const int32_t* q_off;      // [C+1] the inputs' class ranges = the slot ranges
+  const int32_t* class_off;  // [C+1] train rows of each class
+  const T* t;
+  int d;
+  const float* center;
+  __nv_bfloat16* pack;
+  int64_t pitch;
+  float* sqnorm;
+  float* rounderr;
+  uint32_t* row_min;
+  int32_t* cand_cnt;
+  SeedParams seed;
+  T* rows;            // [m x d] the slots' winning train rows (zero row for the no-winner slot)
+  int32_t* slot_class;  // [m] c for a live slot, -1 past k_c (the re-rank writes "no row" there)
+  int32_t* live_end;    // [m] q_off[c] + k_c for every slot of class c (tip_nn_filter_live)
+  int32_t* k;           // [C] distinct winners of each class (+1 if some input has none)
+  int32_t* slot;        // [m] slot of every input
+};
+
+template <typename T>
+__global__ void __launch_bounds__(kCompactThreads) dsa_compact_kernel(const CompactArgs<T> a) {
+  extern __shared__ uint32_t s_words[];   // [W] winner bits, then [W] exclusive prefix of their popcounts
+  __shared__ int s_warp[kCompactThreads / 32];
+  __shared__ int s_none;
+  const int c = blockIdx.x, p = blockIdx.y, P = gridDim.y;
+  const int q0 = a.q_off[c], q1 = a.q_off[c + 1];
+  if (q0 >= q1) return;
+  const int t0 = a.class_off[c], nc = a.class_off[c + 1] - t0;
+  const int W = (nc + 31) >> 5;
+  uint32_t* bits = s_words;
+  int* pre = reinterpret_cast<int*>(s_words + W);
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  for (int w = tid; w < W; w += kCompactThreads) bits[w] = 0u;
+  if (tid == 0) s_none = 0;
+  __syncthreads();
+  for (int i = q0 + tid; i < q1; i += kCompactThreads) {
+    const int j = a.pos[i] - t0;
+    if (j >= 0 && j < nc) atomicOr(bits + (j >> 5), 1u << (j & 31));
+    else s_none = 1;
+  }
+  __syncthreads();
+  // exclusive prefix of the word popcounts: a contiguous run of words per thread, then a block scan of the runs
+  const int per = (W + kCompactThreads - 1) / kCompactThreads;
+  const int w0 = min(W, tid * per), w1 = min(W, w0 + per);
+  int run = 0;
+  for (int w = w0; w < w1; w++) run += __popc(bits[w]);
+  int incl = run;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int v = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += v;
+  }
+  if (lane == 31) s_warp[warp] = incl;
+  __syncthreads();
+  int before = 0, total = 0;
+  for (int w = 0; w < kCompactThreads / 32; w++) {
+    before += w < warp ? s_warp[w] : 0;
+    total += s_warp[w];
+  }
+  int acc = before + incl - run;
+  for (int w = w0; w < w1; w++) {
+    pre[w] = acc;
+    acc += __popc(bits[w]);
+  }
+  __syncthreads();
+  const int kc = total + s_none;
+  if (p == 0 && tid == 0) a.k[c] = kc;
+  // this block's share of the class's slots (live bound, class) and inputs (slot)
+  for (int i = q0 + p * kCompactThreads + tid; i < q1; i += P * kCompactThreads) {
+    a.live_end[i] = q0 + kc;
+    a.slot_class[i] = i - q0 < kc ? c : -1;
+    if (i - q0 >= kc) a.cand_cnt[i] = 0;   // a slot without a query has no candidates
+    const int j = a.pos[i] - t0;
+    int r = total;
+    if (j >= 0 && j < nc) r = pre[j >> 5] + __popc(bits[j >> 5] & ((1u << (j & 31)) - 1u));
+    a.slot[i] = q0 + r;
+  }
+  // one warp per distinct winner: rank r -> its word (binary search over the prefix) -> its bit
+  for (int r = p * (kCompactThreads / 32) + warp; r < kc; r += P * (kCompactThreads / 32)) {
+    int pos = -1;
+    if (r < total) {
+      int lo = 0, hi = W - 1;   // last word with pre[w] <= r
+      while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (pre[mid] <= r) lo = mid;
+        else hi = mid - 1;
+      }
+      uint32_t word = bits[lo];
+      for (int skip = r - pre[lo]; skip > 0; skip--) word &= word - 1u;
+      pos = t0 + 32 * lo + __ffs(word) - 1;
+    }
+    const int64_t s = q0 + r;
+    const T* src = pos >= 0 ? a.t + (int64_t)pos * a.d : nullptr;
+    T* dst = a.rows + s * (int64_t)a.d;
+    for (int e = lane; e < a.d; e += 32) dst[e] = src ? src[e] : (T)0;
+    warp_pack_query<T>(src, a.d, a.center, a.pack + s * a.pitch, a.pitch, a.sqnorm + s, a.rounderr + s, a.row_min + s,
+                       a.cand_cnt + s, lane, (a.seed.ub && pos >= 0) ? a.seed.ub[pos] : __int_as_float(0x7f800000),
+                       &a.seed);
+  }
+}
+
+// dist_b of every input from its slot's search; with out != NULL also the result scatter of write_result's fin_*
+template <typename T>
+__global__ void dsa_slot_out_kernel(const T* slot_dist, const int32_t* slot, int64_t m, const T* dist_a,
+                                    const int32_t* gid, const int32_t* idx, int64_t n_total, T* dist_b, double* out) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= m) return;
+  const T b = slot_dist[slot[i]];
+  dist_b[i] = b;
+  if (!out) return;
+  const int64_t j = idx ? idx[i] : i;
+  if (j < 0 || j >= n_total) return;
+  const T da = dist_a[i];
+  out[j] = (double)da;
+  out[n_total + j] = (double)b;
+  out[2 * n_total + j] = (double)gid[i];
+  out[3 * n_total + j] = (double)Rn<T>::div(da, b);
+}
+
 }  // namespace tip
 
 using namespace tip;
@@ -489,4 +622,65 @@ extern "C" int tip_nn_rerank(const void* q, const void* t, int dtype, int64_t m,
     return launch_rerank<double>(a, st);
   }
   TIP_REQUIRE(false, "dtype must be TIP_F32 or TIP_F64");
+}
+
+extern "C" int64_t tip_dsa_distinct_smem_bytes(int64_t max_class_rows) {
+  if (max_class_rows < 0) return -1;
+  return 8 * ((max_class_rows + 31) / 32);
+}
+
+extern "C" int tip_dsa_distinct_winners(const int32_t* pos, int64_t m, const int32_t* q_off, const int32_t* class_off,
+                                        int32_t n_classes, int64_t max_class_rows, int32_t blocks_per_class,
+                                        const void* t, int dtype, int64_t d, const float* center, const float* seed_ub,
+                                        float t_rmax, float t_errmax, void* rows, void* q_pack, float* q_sqnorm,
+                                        float* q_rounderr, uint32_t* row_min_bits, int32_t* cand_cnt,
+                                        int32_t* slot_class, int32_t* live_end, int32_t* k, int32_t* slot,
+                                        void* stream) {
+  TIP_REQUIRE(pos && q_off && class_off && t && rows && q_pack && q_sqnorm && q_rounderr && row_min_bits && cand_cnt &&
+              slot_class && live_end && k && slot, "null pointer");
+  TIP_REQUIRE(m >= 0 && m < (1LL << 31) && d >= 1 && d < (1LL << 24) && n_classes >= 1 && n_classes < 65536, "shape");
+  TIP_REQUIRE(blocks_per_class >= 1 && blocks_per_class <= 65535, "blocks_per_class");
+  const int64_t smem = tip_dsa_distinct_smem_bytes(max_class_rows);
+  TIP_REQUIRE(smem >= 0 && smem <= 48 * 1024, "max_class_rows: the winner bits of a class must fit in 48 KB");
+  if (m == 0) return TIP_OK;
+  const int64_t pitch = tip_pair_pitch(d, 1);
+  const SeedParams seed{seed_ub, t_rmax, t_errmax, (float)(next_pitch_k16(d) * 16 + 16) * 1.1920929e-7f};
+  const dim3 grid((unsigned)n_classes, (unsigned)blocks_per_class);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (dtype == TIP_F32) {
+    const CompactArgs<float> a{pos, q_off, class_off, (const float*)t, (int)d, center, (__nv_bfloat16*)q_pack, pitch,
+                               q_sqnorm, q_rounderr, row_min_bits, cand_cnt, seed, (float*)rows, slot_class, live_end,
+                               k, slot};
+    dsa_compact_kernel<float><<<grid, kCompactThreads, (size_t)smem, st>>>(a);
+  } else if (dtype == TIP_F64) {
+    const CompactArgs<double> a{pos, q_off, class_off, (const double*)t, (int)d, center, (__nv_bfloat16*)q_pack, pitch,
+                                q_sqnorm, q_rounderr, row_min_bits, cand_cnt, seed, (double*)rows, slot_class, live_end,
+                                k, slot};
+    dsa_compact_kernel<double><<<grid, kCompactThreads, (size_t)smem, st>>>(a);
+  } else {
+    TIP_REQUIRE(false, "dtype must be TIP_F32 or TIP_F64");
+  }
+  TIP_LAUNCH_CHECK();
+  return TIP_OK;
+}
+
+extern "C" int tip_dsa_slot_out(const void* slot_dist, int dtype, const int32_t* slot, int64_t m, const void* dist_a,
+                                const int32_t* gid, const int32_t* idx, int64_t n_total, void* dist_b, double* out,
+                                void* stream) {
+  TIP_REQUIRE(slot_dist && slot && dist_b, "null pointer");
+  TIP_REQUIRE(out == nullptr || (dist_a && gid), "result scatter: dist_a and gid");
+  TIP_REQUIRE(m >= 0 && n_total >= 0, "shape");
+  if (m == 0) return TIP_OK;
+  const unsigned blocks = (unsigned)((m + 255) / 256);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (dtype == TIP_F32)
+    dsa_slot_out_kernel<float><<<blocks, 256, 0, st>>>((const float*)slot_dist, slot, m, (const float*)dist_a, gid, idx,
+                                                       n_total, (float*)dist_b, out);
+  else if (dtype == TIP_F64)
+    dsa_slot_out_kernel<double><<<blocks, 256, 0, st>>>((const double*)slot_dist, slot, m, (const double*)dist_a, gid,
+                                                        idx, n_total, (double*)dist_b, out);
+  else
+    TIP_REQUIRE(false, "dtype must be TIP_F32 or TIP_F64");
+  TIP_LAUNCH_CHECK();
+  return TIP_OK;
 }

@@ -32,6 +32,7 @@ from . import _lib
 POOL_FRAC = 0.2           # share of the filter's work handed out dynamically
 POOL_MIN_TILES = 32       # tiles per CTA below which work lists stay purely static
 POOL_TILES = 4            # train tiles per dynamic item
+LIVE_ITEM_TILES = 16      # train tiles per item of a live-bounded filter (DSA's stage 2 on distinct winners)
 DEFAULT_CAP = 64          # candidate chunks per query (short traces)
 DEFAULT_CAP_LONG = 256    # long traces: distances concentrate, more rows fall inside the window
 
@@ -328,6 +329,26 @@ def build_balanced_items(tiles, col_tile: int, n_cta: int, item_cost: float = 0.
     return np.asarray(out, dtype=np.int32).reshape(-1, 6), n_static
 
 
+def build_live_items(q_off: np.ndarray, ranges_per_class, row_tile: int, col_tile: int,
+                     item_tiles: int = LIVE_ITEM_TILES) -> np.ndarray:
+    """Work list of a filter whose queries end at a bound only the device knows (tip_nn_filter_live: DSA's stage 2
+    on the distinct stage-1 winners, which fill each class's slot range from its start).  Every item is drawn from
+    the pool (n_static = 0) and covers one class-aligned query tile x at most `item_tiles` train tiles.  Items are
+    ordered by the query tile's index inside its class, then class, then train row: the first tiles of every class
+    are the likeliest to hold live rows, so live work comes first and the items past the bounds cluster at the end,
+    where skipping them only costs CTAs that have nothing left to do."""
+    q_off = np.asarray(q_off, dtype=np.int64)
+    width = item_tiles * col_tile
+    keyed = []
+    for c, ranges in enumerate(ranges_per_class):
+        spans = [(s0, min(s0 + width, int(hi))) for lo, hi in ranges for s0 in range(int(lo), int(hi), width)]
+        for j, r0 in enumerate(range(int(q_off[c]), int(q_off[c + 1]), row_tile)):
+            nr = min(row_tile, int(q_off[c + 1]) - r0)
+            keyed.extend(((j, c, s0), (r0, nr, s0, s1, 0, 0)) for s0, s1 in spans)
+    keyed.sort(key=lambda kv: kv[0])
+    return np.asarray([it for _, it in keyed], dtype=np.int32).reshape(-1, 6)
+
+
 def span_major(items: np.ndarray) -> np.ndarray:
     """Order the streaming kernel's work list by (train span, query tile).  CTA b runs items b, b + G, ...,
     so the CTAs that run at the same time then scan the SAME train rows for different query tiles: a train
@@ -606,6 +627,8 @@ class NnEngine:
         self.class_off = np.asarray(class_off, dtype=np.int64)
         self.num_classes = self.class_off.shape[0] - 1
         self.class_off_dev = torch.from_numpy(self.class_off.astype(np.int32)).to(self.dev)
+        self.max_class_rows = int(np.diff(self.class_off).max()) if self.num_classes > 0 else 0
+        self._q_off_dev = {}
         self.t_gid = t_gid.to(torch.int32).contiguous()
         self.cap = int(cap) if cap else (DEFAULT_CAP if self.d <= 256 else DEFAULT_CAP_LONG)
         self.pitch = int(self.lib.tip_pair_pitch(self.d, 1))
@@ -753,6 +776,45 @@ class NnEngine:
                 torch.empty(m, dtype=torch.int32, device=self.dev),
                 torch.empty(m, dtype=torch.int32, device=self.dev))
 
+    def other_class_mixed(self, q_off: np.ndarray, m: int) -> bool:
+        """Few queries per class: the other-class stage tiles across class boundaries (full tiles) and masks each
+        query's own class; many: class-aligned tiles never touch their own class's rows."""
+        populated = int(np.count_nonzero(np.diff(np.asarray(q_off))))
+        return m < 2 * self.row_tile * max(1, populated)
+
+    def distinct_ok(self, q_off: np.ndarray, m: int) -> bool:
+        """True if DSA's stage 2 runs once per distinct stage-1 winner (dsa_distances): the resident-query filter on
+        class-aligned tiles, and every class's winner bits fit tip_dsa_distinct_winners' shared memory."""
+        return (self.resident and not self.other_class_mixed(q_off, m)
+                and 0 <= int(self.lib.tip_dsa_distinct_smem_bytes(self.max_class_rows)) <= 48 * 1024)
+
+    def distinct_winners(self, pos: torch.Tensor, q_off: np.ndarray):
+        """Stage-1 winner positions of class-sorted inputs -> the stage-2 queries once per distinct winner
+        (tip_dsa_distinct_winners): (rows, packed query state, slot_class, live_end, k, slot)."""
+        m = pos.shape[0]
+        key = np.asarray(q_off, dtype=np.int64).tobytes()
+        q_off_dev = self._q_off_dev.get(key)
+        if q_off_dev is None:
+            if len(self._q_off_dev) > 64:
+                self._q_off_dev.clear()
+            q_off_dev = torch.from_numpy(np.asarray(q_off, dtype=np.int32)).to(self.dev)
+            self._q_off_dev[key] = q_off_dev
+        if self._capture_refs is not None:
+            self._capture_refs.extend(t for t in (q_off_dev, self.seed_b) if t is not None)
+        rows = torch.empty((m, self.d), dtype=self.t.dtype, device=self.dev)
+        state = self.query_state(m)
+        slot_class, live_end, slot = (torch.empty(m, dtype=torch.int32, device=self.dev) for _ in range(3))
+        k = torch.empty(self.num_classes, dtype=torch.int32, device=self.dev)
+        per_class = int(np.diff(np.asarray(q_off, dtype=np.int64)).max()) if m else 0
+        q_pack, q_sq, q_err, row_min, cand_cnt = state
+        _lib.check(self.lib.tip_dsa_distinct_winners(_p(pos), m, _p(q_off_dev), _p(self.class_off_dev), self.num_classes,
+                                                     self.max_class_rows, max(1, -(-per_class // 32)), _p(self.t),
+                                                     self.dtype, self.d, _p(self.center), _p(self.seed_b), self.rmax,
+                                                     self.errmax, _p(rows), _p(q_pack), _p(q_sq), _p(q_err), _p(row_min),
+                                                     _p(cand_cnt), _p(slot_class), _p(live_end), _p(k), _p(slot),
+                                                     _stream()), "tip_dsa_distinct_winners")
+        return rows, state, slot_class, live_end, k, slot
+
     def has_items(self, q_off: np.ndarray, mode: int) -> bool:
         """True if a search of this mode would launch the filter for queries with this class histogram."""
         if self.n == 0:
@@ -763,7 +825,7 @@ class NnEngine:
 
     def search(self, q: torch.Tensor, q_class: torch.Tensor, q_off: np.ndarray, mode: int, use_filter: bool = True,
                want_rows: bool = False, prepacked=None, next_query=None, q_idx: Optional[torch.Tensor] = None, fin=None,
-               speculative: bool = False):
+               speculative: bool = False, live_end: Optional[torch.Tensor] = None):
         """q: [m, d] queries grouped by class (q_off), q_class[m] int32.  Returns, per query, the
         exact NumPy-order distance to its nearest train row in the range selected by `mode`
         (NaN when the range is empty on this shard), that row's position (-1 when empty), its
@@ -773,7 +835,9 @@ class NnEngine:
         q_idx: int32 [m] — the queries are rows q_idx[r] of q (class-sorted order over the caller's buffer; no gathered
         copy); fin: (dist_a, gid, idx, n_total, out) — fused result scatter of DSA's last stage (tip_rerank_extras).
         speculative: queries whose candidate list is empty or overflowed are only counted in work_buffer(m)[0] (no
-        exhaustive-scan launch); the caller checks overflow_count() and repeats the call without it if non-zero."""
+        exhaustive-scan launch); the caller checks overflow_count() and repeats the call without it if non-zero.
+        live_end: int32 [m] (distinct_winners) — query rows at and past live_end[r] hold no query; the filter draws
+        every item from its pool and skips the query tiles without live rows (tip_nn_filter_live)."""
         m = q.shape[0] if q_idx is None else q_idx.shape[0]
         use_filter = use_filter and self.filter_ok
         out_dist = torch.empty(m, dtype=q.dtype, device=self.dev)
@@ -786,14 +850,14 @@ class NnEngine:
         cand_idx = cand_cnt = None
         if use_filter and self.n > 0:
             ranges = self.ranges(mode)
-            key = (mode, np.asarray(q_off, dtype=np.int64).tobytes())
+            key = (mode, np.asarray(q_off, dtype=np.int64).tobytes(), live_end is not None)
             plan = self._item_cache.get(key)
             if plan is None:       # host planning + upload once per (mode, class histogram)
-                populated = int(np.count_nonzero(np.diff(np.asarray(q_off))))
-                # few queries per class: tile across class boundaries (full tiles), per-query masking;
-                # many: class-aligned tiles never touch their own class's rows
-                mixed = mode == _lib.RANGE_OTHER_CLASSES and m < 2 * self.row_tile * max(1, populated)
-                if self.resident:
+                mixed = mode == _lib.RANGE_OTHER_CLASSES and self.other_class_mixed(q_off, m)
+                if live_end is not None:
+                    assert self.resident and not mixed
+                    items, n_static = build_live_items(q_off, ranges, self.row_tile, self.col_tile), 0
+                elif self.resident:
                     # resident-query kernel: one or two long items per CTA, equal tile counts
                     tiles = query_tiles(q_off, ranges, self.class_off, self.row_tile, mixed)
                     items, n_static = build_balanced_items(tiles, self.col_tile, self.sms, pool_frac=POOL_FRAC,
@@ -830,13 +894,13 @@ class NnEngine:
                 if PROFILE is not None:
                     ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
                     ev[0].record()
-                _lib.check(lib.tip_nn_filter(_p(q_pack), _p(q_sq), m, _p(self.t_pack), self.n, self.d, self.pitch,
-                                             _p(items_dev), n_items, _p(q_class if flagged else None),
-                                             _p(self.class_off_dev if flagged else None), self.rmax,
-                                             _p(q_err), self.errmax, _p(row_min), _p(cand_idx),
-                                             _p(cand_cnt), self.cap, n_static,
-                                             _p(self.sched_counter if n_static < n_items else None),
-                                             _stream()), "tip_nn_filter")
+                _lib.check(lib.tip_nn_filter_live(_p(q_pack), _p(q_sq), m, _p(self.t_pack), self.n, self.d, self.pitch,
+                                                  _p(items_dev), n_items, _p(q_class if flagged else None),
+                                                  _p(self.class_off_dev if flagged else None), self.rmax,
+                                                  _p(q_err), self.errmax, _p(row_min), _p(cand_idx),
+                                                  _p(cand_cnt), self.cap, n_static,
+                                                  _p(self.sched_counter if n_static < n_items else None),
+                                                  _p(live_end), _stream()), "tip_nn_filter_live")
                 if ev is not None:
                     ev[1].record()
                     name = "nn_filter_same_class" if mode == _lib.RANGE_SAME_CLASS else "nn_filter_other_classes"
@@ -923,8 +987,22 @@ def dsa_distances(engine: NnEngine, x: torch.Tensor, q_class: torch.Tensor, q_of
                                                    m, int(scatter[1]), _p(scatter[2]), _stream()), "tip_dsa_pack_out")
         return dist_a, dist_b, gid
     if not sharded:
-        # single shard: stage 1's re-rank also emits its winners as the packed queries of stage 2
         fuse = use_filter and engine.has_items(q_off, _lib.RANGE_OTHER_CLASSES)
+        if fuse and engine.distinct_ok(q_off, m):
+            # stage 2 depends on the input only through its stage-1 winner: search once per distinct winner (slots in
+            # training-row order inside each class's range), then hand every input its slot's dist_b
+            dist_a, pos, gid, _ = engine.search(x, q_class, q_off, _lib.RANGE_SAME_CLASS, use_filter, q_idx=q_idx,
+                                                speculative=speculative)
+            rows, state2, slot_class, live_end, _, slot = engine.distinct_winners(pos, q_off)
+            slot_b = engine.search(rows, slot_class, q_off, _lib.RANGE_OTHER_CLASSES, use_filter, prepacked=state2,
+                                   live_end=live_end, speculative=speculative)[0]
+            dist_b = torch.empty_like(dist_a)
+            idx, n_total, out = (None, 0, None) if scatter is None else scatter
+            _lib.check(engine.lib.tip_dsa_slot_out(_p(slot_b), tip_dtype(slot_b.dtype), _p(slot), m, _p(dist_a), _p(gid),
+                                                   _p(idx), int(n_total), _p(dist_b), _p(out), _stream()),
+                       "tip_dsa_slot_out")
+            return dist_a, dist_b, gid
+        # single shard: stage 1's re-rank also emits its winners as the packed queries of stage 2
         state2 = engine.query_state(m) if fuse else None
         dist_a, _, gid, winners = engine.search(x, q_class, q_off, _lib.RANGE_SAME_CLASS, use_filter, want_rows=True,
                                                 next_query=state2, q_idx=q_idx, speculative=speculative)

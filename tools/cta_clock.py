@@ -19,14 +19,26 @@ order, q_off = E.class_layout(pte, 10)
 x = E.to_device(xte, eng.dev).index_select(0, torch.from_numpy(order).to(eng.dev))
 qc = torch.from_numpy(pte[order].astype(np.int32)).to(eng.dev)
 lib = _lib.load()
-w = eng.gather(eng.search(x, qc, q_off, _lib.RANGE_SAME_CLASS)[1])
-for mode, q in ((_lib.RANGE_OTHER_CLASSES, w), (_lib.RANGE_SAME_CLASS, x)):
+_, pos, _, _ = eng.search(x, qc, q_off, _lib.RANGE_SAME_CLASS)
+w = eng.gather(pos)
+
+
+def distinct():
+    # DSA's stage 2 as dsa_distances runs it: once per distinct winner, live-bounded work list drawn from the pool
+    rows, state, slot_class, live_end, _, _ = eng.distinct_winners(pos, q_off)
+    eng.search(rows, slot_class, q_off, _lib.RANGE_OTHER_CLASSES, prepacked=state, live_end=live_end)
+
+
+runs = [("other classes, every input", _lib.RANGE_OTHER_CLASSES, lambda: eng.search(w, qc, q_off, _lib.RANGE_OTHER_CLASSES)),
+        ("other classes, distinct winners", _lib.RANGE_OTHER_CLASSES, distinct),
+        ("same class", _lib.RANGE_SAME_CLASS, lambda: eng.search(x, qc, q_off, _lib.RANGE_SAME_CLASS))]
+for label, mode, run in runs:
     for _ in range(2):
-        eng.search(q, qc, q_off, mode)
+        run()
     buf = torch.zeros((320, 4), dtype=torch.int64, device=eng.dev)     # rows 0..255: per-CTA records, 256..: entry times
     lib.tip_debug_cta_clock(C.c_void_p(buf.data_ptr()))
     E.PROFILE = []
-    eng.search(q, qc, q_off, mode)
+    run()
     torch.cuda.synchronize()
     prof, E.PROFILE = E.PROFILE, None
     lib.tip_debug_cta_clock(None)
@@ -34,7 +46,7 @@ for mode, q in ((_lib.RANGE_OTHER_CLASSES, w), (_lib.RANGE_SAME_CLASS, x)):
     entry = raw.reshape(-1)[1024:1024 + 148]
     t = raw[:256]
     pro = (t[:148, 0] - entry) / 1e3
-    print(f"mode {mode}: kernel entry -> post-allocation timestamp per CTA: min {pro.min():.2f} p50 {np.median(pro):.2f} max {pro.max():.2f} us; "
+    print(f"{label}: kernel entry -> post-allocation timestamp per CTA: min {pro.min():.2f} p50 {np.median(pro):.2f} max {pro.max():.2f} us; "
           f"entry skew across CTAs {(entry.max() - entry.min()) / 1e3:.2f} us; first entry -> last CTA end {(t[:148, 1].max() - entry.min()) / 1e3:.1f} us; "
           f"event-timed launches: {[(k, round(a.elapsed_time(b) * 1e3, 1)) for k, _, a, b in prof] if prof else None}")
     t = t[t[:, 1] > 0]
@@ -43,7 +55,7 @@ for mode, q in ((_lib.RANGE_OTHER_CLASSES, w), (_lib.RANGE_SAME_CLASS, x)):
     t0 = t[:, 0].min()
     start, end = (t[:, 0] - t0) / 1e3, (t[:, 1] - t0) / 1e3
     dur = end - start
-    print(f"mode {mode}: {len(t)} CTAs; kernel span {end.max():.1f} us; CTA start skew max {start.max():.1f} us; "
+    print(f"{label}: {len(t)} CTAs; kernel span {end.max():.1f} us; CTA start skew max {start.max():.1f} us; "
           f"CTA duration min {dur.min():.1f} p50 {np.median(dur):.1f} p90 {np.percentile(dur, 90):.1f} max {dur.max():.1f} us")
     print(f"  tiles per CTA min {t[:, 2].min()} p50 {np.median(t[:, 2]):.0f} max {t[:, 2].max()}; items per CTA min {items.min()} max {items.max()}")
     print(f"  ns per tile: min {np.min(dur * 1e3 / t[:, 2]):.0f} p50 {np.median(dur * 1e3 / t[:, 2]):.0f} max {np.max(dur * 1e3 / t[:, 2]):.0f}")
