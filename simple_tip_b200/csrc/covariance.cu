@@ -87,78 +87,22 @@ __global__ void __launch_bounds__(kCovThreads) cov_location_kernel(const T* __re
   var[c] = cov_div<T>(s2, n);
 }
 
-// one leaf [o, o + n) (n <= 128) of NumPy's pairwise sum of term(i), accumulated in A
-template <typename A, typename F>
-__device__ A cov_leaf(const F& term, int o, int n) {
-  using R = Rn<A>;
-  if (n < 8) {
-    A res = (A)0;
-    for (int i = 0; i < n; i++) res = R::add(res, term(o + i));
-    return res;
-  }
-  A r[8];
-#pragma unroll
-  for (int j = 0; j < 8; j++) r[j] = term(o + j);
-  int i = 8;
-  const int lim = n - (n % 8);
-  for (; i < lim; i += 8)
-#pragma unroll
-    for (int j = 0; j < 8; j++) r[j] = R::add(r[j], term(o + i + j));
-  A res = R::add(R::add(R::add(r[0], r[1]), R::add(r[2], r[3])), R::add(R::add(r[4], r[5]), R::add(r[6], r[7])));
-  for (; i < n; i++) res = R::add(res, term(o + i));
-  return res;
-}
-
-// NumPy's pairwise sum of term(0 .. n-1) accumulated in A, with an explicit stack (depth <= 32 for n < 2^31)
-template <typename A, typename F>
-__device__ A cov_pairwise(const F& term, int n) {
-  if (n <= 128) return cov_leaf<A>(term, 0, n);
-  int off[32], len[32];
-  unsigned char phase[32];
-  A vals[32];
-  int sp = 1, vp = 0;
-  off[0] = 0; len[0] = n; phase[0] = 0;
-  while (sp > 0) {
-    const int top = sp - 1;
-    const int o = off[top], l = len[top];
-    if (l <= 128) {
-      vals[vp++] = cov_leaf<A>(term, o, l);
-      sp--;
-      continue;
-    }
-    const int n2 = l / 2 - (l / 2) % 8;
-    if (phase[top] == 0) {
-      phase[top] = 1;
-      off[sp] = o; len[sp] = n2; phase[sp] = 0; sp++;
-    } else if (phase[top] == 1) {
-      phase[top] = 2;
-      off[sp] = o + n2; len[sp] = l - n2; phase[sp] = 0; sp++;
-    } else {
-      const A rgt = vals[--vp];
-      const A lft = vals[--vp];
-      vals[vp++] = Rn<A>::add(lft, rgt);
-      sp--;
-    }
-  }
-  return vals[0];
-}
-
 template <typename T>
 __global__ void cov_location_1d_kernel(const T* __restrict__ x, int64_t n, T* __restrict__ loc,
                                        double* __restrict__ mean, T* __restrict__ var, int32_t* __restrict__ flags) {
   int flag = 0;
   for (int64_t i = 0; i < n; i++) flag |= cov_flag((double)x[i]);
   // the reduce adds the pairwise sum to the identity 0 (this also turns a -0 sum into +0, as NumPy does)
-  const T m = cov_div<T>(Rn<T>::add((T)0, cov_pairwise<T>([&](int i) { return x[i]; }, (int)n)), n);
+  const T m = cov_div<T>(Rn<T>::add((T)0, np_sum<T>([&](int i) { return x[i]; }, (int)n)), n);
   if (loc) loc[0] = m;
-  mean[0] = __ddiv_rn(__dadd_rn(0.0, cov_pairwise<double>([&](int i) { return (double)x[i]; }, (int)n)), (double)n);
+  mean[0] = __ddiv_rn(__dadd_rn(0.0, np_sum<double>([&](int i) { return (double)x[i]; }, (int)n)), (double)n);
   *flags = flag;
   if (var) {
     const auto sq = [&](int i) {
       const T e = Rn<T>::sub(x[i], m);
       return Rn<T>::mul(e, e);
     };
-    var[0] = cov_div<T>(Rn<T>::add((T)0, cov_pairwise<T>(sq, (int)n)), n);
+    var[0] = cov_div<T>(Rn<T>::add((T)0, np_sum<T>(sq, (int)n)), n);
   }
 }
 

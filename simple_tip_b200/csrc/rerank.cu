@@ -17,9 +17,6 @@
 // Both also emit the winner's original index and (optionally) copy the winning train row, which
 // is the query of DSA's second stage (surprise.py:627-629, 648).
 #include <algorithm>
-#include <map>
-#include <mutex>
-#include <vector>
 #include "common.cuh"
 
 namespace tip {
@@ -98,6 +95,19 @@ struct RerankArgs {
 template <typename T>
 __device__ __forceinline__ const T* query_row(const RerankArgs<T>& a, int64_t row) {
   return a.q + (a.q_idx ? (int64_t)a.q_idx[row] : row) * (int64_t)a.d;
+}
+
+// sum of (x-y)^2 over the trace in NumPy's pairwise order, by the calling 8-lane group: the leaf program of width d,
+// or the recursion for widths it cannot encode
+template <typename T>
+__device__ __forceinline__ T group_sumsq(const RerankArgs<T>& a, const T* __restrict__ x, const T* __restrict__ y,
+                                         int sub, unsigned gmask) {
+  const auto term = [&](int i) {
+    const T d = Rn<T>::sub(x[i], y[i]);
+    return Rn<T>::mul(d, d);
+  };
+  if (a.sum_prog) return np_sum_prog_g8<T>(term, a.sum_prog, a.sum_leaves, sub, gmask);
+  return np_pairwise<T>([&](int o, int l) { return np_leaf_sum_g8<T>(term, o, l, sub, gmask); }, a.d);
 }
 
 template <typename T>
@@ -231,8 +241,7 @@ rerank_list_kernel(const RerankArgs<T> a) {
           }
           s = r;
         } else {
-          s = a.sum_prog ? np_sumsq_prog_g8<T>(x, y, a.sum_prog, a.sum_leaves, sub, gmask)
-                         : np_sumsq_g8<T>(x, y, a.d, sub, gmask);
+          s = group_sumsq(a, x, y, sub, gmask);
         }
         const bool in_range = a.mode == TIP_RANGE_SAME_CLASS ? (j >= c0 && j < c1) : (j < cn && (j < c0 || j >= c1));
         if (in_range) consider(best, Rn<T>::sqrt(s), gid, j);   // all 8 lanes agree
@@ -335,8 +344,7 @@ __global__ void __launch_bounds__(kScanThreads) rerank_scan_kernel(const RerankA
     const int64_t lo = total * sl / S, hi = total * (sl + 1) / S;
     for (int64_t li = lo + grp; li < hi; li += kGroups) {
       const int j = li < len0 ? base0 + (int)li : c1 + (int)(li - len0);
-      const T s = a.sum_prog ? np_sumsq_prog_g8<T>(x, a.t + (int64_t)j * a.d, a.sum_prog, a.sum_leaves, sub, gmask)
-                             : np_sumsq_g8<T>(x, a.t + (int64_t)j * a.d, a.d, sub, gmask);
+      const T s = group_sumsq(a, x, a.t + (int64_t)j * a.d, sub, gmask);
       consider(best, Rn<T>::sqrt(s), a.t_gid ? a.t_gid[j] : j, j);
     }
     if (sub == 0) { s_dist[grp] = best.dist; s_gid[grp] = best.gid; s_pos[grp] = best.pos; }
@@ -524,47 +532,6 @@ static int next_pitch_k16(int64_t d) {     // K=16 steps of the one-segment pack
   return (int)((d16 + 16) / 16);
 }
 
-// NumPy's pairwise schedule for width d as one word per leaf (common.cuh: np_sumsq_prog_g8), cached per
-// (device, d) in device memory.  Built outside stream capture: the first search of an engine is eager.
-static void build_sum_prog(int off, int n, std::vector<uint32_t>& prog) {
-  if (n <= 128) {
-    prog.push_back((uint32_t)(off / 8) | ((uint32_t)(n - 1) << 20));
-    return;
-  }
-  int n2 = n / 2;
-  n2 -= n2 % 8;
-  build_sum_prog(off, n2, prog);
-  build_sum_prog(off + n2, n - n2, prog);
-  prog.back() += 1u << 27;          // after the right subtree: merge it with the left one
-}
-
-static int get_sum_prog(int64_t d, const uint32_t** dev_prog, int* n_leaves) {
-  static std::mutex mu;
-  static std::map<std::pair<int, int64_t>, std::pair<uint32_t*, int>> cache;
-  *dev_prog = nullptr;
-  *n_leaves = 0;
-  if (d <= 128 || d > (8LL << 20)) return TIP_OK;      // short traces: register-resident leaf; absurd widths: generic routine
-  int dev = 0;
-  TIP_CHECK_CUDA(cudaGetDevice(&dev));
-  std::lock_guard<std::mutex> lock(mu);
-  auto it = cache.find({dev, d});
-  if (it == cache.end()) {
-    std::vector<uint32_t> prog;
-    build_sum_prog(0, (int)d, prog);
-    for (uint32_t w : prog)
-      if ((w >> 27) >= 31) return TIP_OK;               // cannot happen below 2^31 elements; fall back if it does
-    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-    uint32_t* p = nullptr;
-    TIP_CHECK_CUDA(cudaMalloc(&p, prog.size() * sizeof(uint32_t)));
-    TIP_CHECK_CUDA(cudaMemcpy(p, prog.data(), prog.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
-    (void)cap;
-    it = cache.emplace(std::make_pair(dev, d), std::make_pair(p, (int)prog.size())).first;
-  }
-  *dev_prog = it->second.first;
-  *n_leaves = it->second.second;
-  return TIP_OK;
-}
-
 extern "C" int32_t tip_sizeof_rerank_extras(void) { return (int32_t)sizeof(tip_rerank_extras); }
 
 extern "C" int64_t tip_nn_rerank_work_bytes(int64_t m, int dtype) {
@@ -597,10 +564,10 @@ extern "C" int tip_nn_rerank(const void* q, const void* t, int dtype, int64_t m,
   const int count_only = ex.count_overflow_only != 0;
   cudaStream_t st = (cudaStream_t)stream;
   const int64_t next_pitch = tip_pair_pitch(d, 1);
-  const uint32_t* sum_prog = nullptr;
+  const uint32_t* sum_prog = nullptr;    // short traces: register-resident leaf; d > kSumProgMaxN: the recursion
   int sum_leaves = 0;
-  {
-    const int rc = get_sum_prog(d, &sum_prog, &sum_leaves);
+  if (d > kPairwiseLeaf && d <= kSumProgMaxN) {
+    const int rc = sum_prog_for(d, &sum_prog, &sum_leaves);
     if (rc != TIP_OK) return rc;
   }
   // gamma of tip_nn_filter for this trace width (packed width + 16 fp32 accumulation steps)
