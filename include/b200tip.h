@@ -251,6 +251,16 @@ int tip_pack_bool(const void* profile_u8, int64_t n, int64_t f, uint32_t* bits, 
 int tip_cam_bits(const uint32_t* bits, int64_t n, int64_t words, int32_t* gain, uint32_t* covered2,
                  int32_t* cand_scratch, int32_t* order, int32_t* state, int32_t max_rounds,
                  int32_t init_gain, void* stream);
+/* tip_cam_bits_stack: tip_cam_bits on the profiles of `models` models at once (a stack's), with one leading
+ * model axis on every buffer but the scratch: bits [models, n, words], gain [models, n], covered2
+ * [models, 2, words] zero-filled, order [models, n], state [models, 4] = {picks, done, -, -} per model,
+ * cand_scratch as for tip_cam_bits.  Slice m of order and state equals tip_cam_bits on bits[m].  Call again
+ * with the same buffers (init_gain = 0) while any model has done == 0 && picks < n; max_rounds must be even
+ * when more calls follow.  models * n < 2^31.  More models than one co-resident grid holds run in consecutive
+ * launches. */
+int tip_cam_bits_stack(const uint32_t* bits, int64_t models, int64_t n, int64_t words, int32_t* gain,
+                       uint32_t* covered2, int32_t* cand_scratch, int32_t* order, int32_t* state,
+                       int32_t max_rounds, int32_t init_gain, void* stream);
 
 /* ---- operand packing for the tensor-core pass ----------------------------------------
  * Packed row (bf16), D16 = round_up(d,16), one 16-wide tail block:

@@ -82,6 +82,7 @@ _SIGNATURES = {
     "tip_stats_update": (C.c_int, [_vp, C.c_int, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp]),
     "tip_pack_bool": (C.c_int, [_vp, _i64, _i64, _vp, _vp]),
     "tip_cam_bits": (C.c_int, [_vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _vp]),
+    "tip_cam_bits_stack": (C.c_int, [_vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _vp]),
     "tip_pair_pitch": (_i64, [_i64, C.c_int]),
     "tip_pair_prep": (C.c_int, [_vp, C.c_int, _i64, _i64, _vp, C.c_int, C.c_int, _f32, _f32, _vp, _vp, _vp, _vp]),
     "tip_nn_filter": (C.c_int, [_vp, _vp, _i64, _vp, _i64, _i64, _i64, _vp, _i32, _vp, _vp, _f32, _vp, _f32, _vp, _vp,

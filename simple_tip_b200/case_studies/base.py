@@ -315,12 +315,16 @@ class CaseStudy:
             os.makedirs(os.path.dirname(path), exist_ok=True)
             torch.save(model.state_dict(), path)
 
-    def run_prio_eval(self, model_ids: Sequence[int], stacked: bool = False,
-                      stack_size: Optional[int] = None) -> Dict[int, dict]:
+    def run_prio_eval(self, model_ids: Sequence[int], stacked: bool = False, stack_size: Optional[int] = None,
+                      stacked_coverage: bool = False) -> Dict[int, dict]:
         """`_prioritization_evaluator` per id: `core.prioritization.evaluate` with the case study's layers and
         badge sizes; returns {model_id: its APFDs}.  stacked=True loads the ids' models and evaluates them in stacks
         of at most `stack_size` (None: all ids in one) with `core.prioritization.evaluate_stack`, which writes the
-        same files and scores the fault predictors of a stack in one pass."""
+        same files and scores the fault predictors of a stack in one pass; stacked_coverage=True (only with
+        stacked=True, ValueError otherwise) runs each stack's coverage arm together too.  A stacked coverage arm
+        holds the stack's test traces, stack_size * N * D * 4 bytes (`StackedCoverageWorker`)."""
+        if stacked_coverage and not stacked:
+            raise ValueError("stacked_coverage=True needs stacked=True")
         res = {}
         if stacked:
             if stack_size is not None and stack_size < 1:
@@ -333,7 +337,7 @@ class CaseStudy:
                     chunk, self.name, [self.load_model(i) for i in chunk], self.train_set[0], self.nominal_set[0],
                     self.nominal_set[1], self.ood_set[0], self.ood_set[1], self.nc_layers, self.sa_layers,
                     dsa_badge_size=self.dsa_badge_size, output_folder=self.output_folder,
-                    batch_size=self.prediction_badge_size))
+                    batch_size=self.prediction_badge_size, stacked_coverage=stacked_coverage))
             return res
         for model_id in model_ids:
             res[model_id] = prioritization.evaluate(

@@ -9,8 +9,9 @@ m's parameters back as `p[m]`, bit for bit.
 
 Layouts: a stack whose first layer is a Conv2D or MaxPooling2D takes its input channel-interleaved, [B, H, W, M * C]
 with channel m * C + c = model m's channel c (`tip_stack_gather`'s interleaved layout), and keeps that layout up to
-its Flatten; every other stack takes its input model-major, [M, B, ...].  `logits(x)` returns [M, B, classes],
-contiguous, the input of `tip_softmax_xent_seg`.  Dropout acts element-wise on the stacked tensor, so each model
+its Flatten; every other stack takes its input model-major, [M, B, ...].  `model_major(child, y)` turns any child's
+output back into [M, B, ...], so callers that read hooked layers never re-derive these layouts.  `logits(x)` returns
+[M, B, classes], contiguous, the input of `tip_softmax_xent_seg`.  Dropout acts element-wise on the stacked tensor, so each model
 draws its own mask.
 """
 from __future__ import annotations
@@ -200,6 +201,21 @@ class StackedSequential(torch.nn.Sequential):
             x = torch.stack(list(xs), dim=3)                     # [B, H, W, M, C]
             return x.reshape(*x.shape[:3], -1)
         return torch.stack(list(xs))
+
+    def model_major(self, child: int, y: torch.Tensor) -> torch.Tensor:
+        """The output y of child `child` as [M, B, *model m's layer shape], slice m being what model m's own layer
+        gives: the inverse of `stack_inputs` for that child's layout.  Children before the Flatten of an
+        interleaved stack give [B, H, W, M * C] (returned as a strided view); every other child gives [M, B, ...]
+        (returned as is).  IndexError for a child index out of range."""
+        children = list(self.children())
+        if not 0 <= child < len(children):
+            raise IndexError(f"child index {child} out of range (the stack has {len(children)} children)")
+        flatten_at = next((i for i, c in enumerate(children) if isinstance(c, StackedFlatten)), len(children))
+        if self.channels_interleaved and child < flatten_at:
+            m = len(self.sources)
+            b, h, w, mc = y.shape
+            return y.reshape(b, h, w, m, mc // m).permute(3, 0, 1, 2, 4)
+        return y
 
     def logits(self, x):
         x = x.to(torch.float32) if self.cast_input else x

@@ -108,6 +108,15 @@ class HookedModelHandler:
 
         return next(iter(self.base_model.model.parameters()), torch.empty(0)).device
 
+    def _inputs(self, data, what: str):
+        """data as a tensor on the model's device; ValueError for an empty set"""
+        import torch
+
+        x = data if isinstance(data, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(data))
+        if x.shape[0] == 0:
+            raise ValueError(f"{what} holds no inputs")
+        return x.to(self._model_device())
+
     def _synced(self, fn, timer):
         """fn() timed by `timer`, which stops after a synchronise of the current CUDA device (the scoring device)
         and of the model's device when that is another CUDA device."""

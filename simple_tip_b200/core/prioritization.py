@@ -13,7 +13,7 @@ APFD.
 from __future__ import annotations
 
 import gc
-from typing import Dict, Optional, Sequence, Tuple
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -81,20 +81,27 @@ def evaluate(model_id: int, case_study: str, model, training_dataset, nominal_te
 def evaluate_stack(model_ids: Sequence[int], case_study: str, models: Sequence, training_dataset,
                    nominal_test_dataset, nominal_test_labels, ood_test_dataset, ood_test_labels,
                    nc_activation_layers: Sequence, sa_activation_layers: Sequence,
-                   dsa_badge_size: Optional[int] = None, output_folder: str = OUTPUT_FOLDER, batch_size: int = 128
-                   ) -> Dict[int, Dict[str, Dict[str, float]]]:
+                   dsa_badge_size: Optional[int] = None, output_folder: str = OUTPUT_FOLDER, batch_size: int = 128,
+                   stacked_coverage: bool = False) -> Dict[int, Dict[str, Dict[str, float]]]:
     """`evaluate` for M models of one architecture (`KerasSequential` networks, model k has id model_ids[k]):
     every file `evaluate(model_ids[k], ..., models[k], ...)` writes, under the same names.
 
     The fault predictors of both datasets come from one `case_studies.stacked.stack(models)`
-    (`activations.get_pred_and_uncertainty_stack`, its defaults as `evaluate` takes the single-model ones); the
-    coverage and the surprise arm then run model by model, in `evaluate`'s order, each arm freed before the next.
+    (`activations.get_pred_and_uncertainty_stack`, its defaults as `evaluate` takes the single-model ones); by default
+    the coverage and the surprise arm then run model by model, in `evaluate`'s order, each arm freed before the next.
     Their score and CAM-order files are those of `evaluate`; the fault predictors' are those of the stacked forward,
     which equals each model's own forward to rounding (the torch sampler's masks differ: see
     `get_pred_and_uncertainty_stack`), and their time files hold each phase's time split evenly over the M models.
 
+    stacked_coverage=True runs the coverage arm on the stack too: one `coverage_worker.StackedCoverageWorker` walks
+    the training set once for all M models and scores both datasets, writing every coverage file `evaluate` writes
+    under the same names.  Its traces are the stacked forward's, so its scores and orders equal `evaluate`'s only as
+    far as that forward's rounding allows, and its time files hold each phase's time split evenly over the M models.
+    The surprise arm still runs model by model.
+
     Returns {model_id: what `evaluate` returns for it}.  ValueError, before any forward pass, for the conditions
-    `evaluate` refuses, for len(models) != len(model_ids) and for repeated model ids."""
+    `evaluate` refuses, for len(models) != len(model_ids), for repeated model ids and, with stacked_coverage, for
+    coverage layers that are not child indices."""
     from ..case_studies.stacked import stack
 
     model_ids = [int(i) for i in model_ids]
@@ -104,6 +111,8 @@ def evaluate_stack(model_ids: Sequence[int], case_study: str, models: Sequence, 
         raise ValueError(f"model ids {model_ids} repeat")
     if "_" in case_study:
         raise ValueError(f"case_study {case_study!r} contains '_', which the result file names cannot carry")
+    if stacked_coverage:
+        coverage_worker.stack_layer_ids(nc_activation_layers)
     labels = {NOM: _flat_labels(nominal_test_labels, nominal_test_dataset, "nominal_test_labels"),
               OOD: _flat_labels(ood_test_labels, ood_test_dataset, "ood_test_labels")}
     datasets = {NOM: nominal_test_dataset, OOD: ood_test_dataset}
@@ -117,14 +126,20 @@ def evaluate_stack(model_ids: Sequence[int], case_study: str, models: Sequence, 
         for model_id, (pred, uncertainties, times) in zip(model_ids, per_model):
             masks[model_id][ds], scores[model_id][ds] = _persist_fault_predictors(
                 output_folder, case_study, model_id, labels[ds], ds, pred, uncertainties, times)
-    del stacked, per_model
+    del per_model
+    stacked_nc = (_eval_neuron_coverage_stack(output_folder, case_study, stacked, model_ids, datasets, training_dataset,
+                                              nc_activation_layers, batch_size) if stacked_coverage else None)
+    del stacked
     gc.collect()
 
     res: Dict[int, Dict[str, Dict[str, float]]] = {}
-    for model_id, model in zip(model_ids, models):
-        nc_scores, nc_orders = _eval_neuron_coverage(output_folder, case_study, model, model_id, datasets,
-                                                     training_dataset, nc_activation_layers, batch_size)
-        gc.collect()
+    for k, (model_id, model) in enumerate(zip(model_ids, models)):
+        if stacked_nc is not None:
+            nc_scores, nc_orders = stacked_nc[k]
+        else:
+            nc_scores, nc_orders = _eval_neuron_coverage(output_folder, case_study, model, model_id, datasets,
+                                                         training_dataset, nc_activation_layers, batch_size)
+            gc.collect()
         sa_scores, sa_orders = _eval_surprise(output_folder, case_study, model, model_id, datasets, training_dataset,
                                               sa_activation_layers, batch_size, dsa_badge_size)
         gc.collect()
@@ -189,6 +204,22 @@ def _eval_neuron_coverage(output_folder, case_study, model, model_id, datasets, 
         scores[ds] = dict(all_scores)
         cam_orders[ds] = {f"{metric}-cam": np.array(order) for metric, order in orders.items()}
     return scores, cam_orders
+
+
+def _eval_neuron_coverage_stack(output_folder, case_study, stacked, model_ids, datasets, training_dataset, layers,
+                                batch_size) -> List[Tuple[Dict[str, Arrays], Dict[str, Arrays]]]:
+    """`_eval_neuron_coverage` for every model of a stack from one `StackedCoverageWorker`: per model (in stack
+    order) its scores and CAM orders per dataset, its files written under its id."""
+    per_model = [({}, {}) for _ in model_ids]
+    nc_worker = coverage_worker.StackedCoverageWorker(stacked, layers, training_dataset, batch_size=batch_size)
+    for ds, x in datasets.items():
+        for (scores, cam_orders), model_id, (times, all_scores, orders) in zip(per_model, model_ids,
+                                                                             nc_worker.evaluate_all(x, ds)):
+            for metric, s in all_scores.items():
+                results.persist_tip(output_folder, case_study, ds, model_id, metric, s, orders[metric], times[metric])
+            scores[ds] = dict(all_scores)
+            cam_orders[ds] = {f"{metric}-cam": np.array(order) for metric, order in orders.items()}
+    return per_model
 
 
 def _eval_surprise(output_folder, case_study, model, model_id, datasets, training_dataset, layers, batch_size,

@@ -2,11 +2,13 @@
 
 `ctm` / `cam` keep the reference's signatures; `cam`'s greedy loop runs on the GPU over the bit-packed
 profile (`cam_from_bits`, one persistent cooperative kernel), which is also the entry point for profiles that
-never left HBM (`NAC/NBC/SNAC/TKNC.packed`).  `cam_from_buckets` is the same ordering for k-multisection profiles given in their compact form
+never left HBM (`NAC/NBC/SNAC/TKNC.packed`); `cam_from_bits_stack` orders the profiles of a model stack's M models
+in one such kernel.  `cam_from_buckets` is the same ordering for k-multisection profiles given in their compact form
 (the bucket ids of `KMNC.buckets`): the greedy loop runs on the GPU (libb200tip `tip_cam_buckets`)
 without ever building the N x D x k array, which is 41 GB at k = 1000.  `cam_from_surprise` is the ordering for
 surprise-coverage profiles (`SurpriseCoverageMapper`): one pass over the scores (libb200tip `tip_sc_cam`)."""
-from typing import Generator
+import itertools
+from typing import Generator, List, Sequence
 
 import numpy as np
 
@@ -79,6 +81,46 @@ def cam_from_bits(scores: np.ndarray, bits, rounds_per_launch: int = 4096) -> Ge
     LAST_GREEDY_PICKS = int(greedy.shape[0])
     yield from (int(i) for i in greedy)
     yield from _tail_by_score(scores, greedy)
+
+
+def cam_from_bits_stack(scores: Sequence[np.ndarray], bits, rounds_per_launch: int = 4096) -> List[np.ndarray]:
+    """`cam_from_bits` for the profiles of M models at once (a model stack's): bits [M, N, words] int32 CUDA tensor,
+    scores M vectors of N.  The M greedy loops run in one persistent cooperative kernel (libb200tip
+    `tip_cam_bits_stack`), one grid barrier per round for all of them; each model's remaining samples then follow
+    by its scores on the host (`_tail_by_score`).  Returns, per model m, the int64 order
+    `list(cam_from_bits(scores[m], bits[m]))` gives."""
+    import torch
+
+    from .. import _lib
+    from .. import engine as E
+
+    scores = [np.asarray(s).copy() for s in scores]
+    assert bits.ndim == 3, "bits [M, N, words]"
+    models, n, words = (int(s) for s in bits.shape)
+    assert len(scores) == models and all(s.ndim == 1 and s.shape[0] == n for s in scores), "M vectors of N scores"
+    greedy = [np.zeros(0, dtype=np.int64)] * models
+    if models > 0 and n > 0 and words > 0:
+        lib = _lib.load()
+        dev = bits.device
+        bits = bits.contiguous()
+        gain = torch.empty((models, n), dtype=torch.int32, device=dev)
+        covered = torch.zeros((models, 2 * words), dtype=torch.int32, device=dev)
+        cand = torch.zeros(4 * _lib.CAM_MAX_BLOCKS, dtype=torch.int32, device=dev)
+        order = torch.zeros((models, n), dtype=torch.int32, device=dev)
+        state = torch.zeros((models, 4), dtype=torch.int32, device=dev)
+        rounds = max(2, int(rounds_per_launch) & ~1)              # even: the covered sets are double-buffered by parity
+        first = 1
+        while True:
+            _lib.check(lib.tip_cam_bits_stack(E._p(bits), models, n, words, E._p(gain), E._p(covered), E._p(cand),
+                                              E._p(order), E._p(state), rounds, first, E._stream()),
+                       "tip_cam_bits_stack")
+            first = 0
+            st = state.cpu().numpy()
+            if not np.any((st[:, 1] == 0) & (st[:, 0] < n)):
+                break
+        picked = order.cpu().numpy()
+        greedy = [picked[m, :st[m, 0]].astype(np.int64) for m in range(models)]
+    return [np.fromiter(itertools.chain(g, _tail_by_score(s, g)), dtype=np.int64) for s, g in zip(scores, greedy)]
 
 
 def pack_profiles(profiles):

@@ -13,6 +13,8 @@
 //                        applied sample by sample in the activation dtype — reproduced bit for bit)
 //   tip_cam_bits         cam() of prioritizers.py:16-45 on bit-packed profiles, one persistent
 //                        cooperative kernel for all greedy rounds
+//   tip_cam_bits_stack   the same for the profiles of a stack of models: one greedy loop per model, all under one
+//                        grid barrier per round
 //
 // All three profile kernels write the reference's dense boolean profile (one byte per entry, what the
 // classes return) and/or the same profile bit-packed for tip_cam_bits.  Packed layout (a fixed
@@ -323,6 +325,119 @@ __global__ void __launch_bounds__(kCamThreads) cam_bits_kernel(const uint32_t* _
   if (blockIdx.x == 0 && threadIdx.x == 0) state[0] = picks;
 }
 
+// ---- CAM for a stack of models: independent greedy loops under one grid barrier per round ----------------------------
+// The grid is cut into gridDim.x / bpm groups of bpm consecutive blocks; group g runs cam_bits_kernel's (A)/(B)/(C) on
+// model g's profile, gains, covered set, order and state.  Every block publishes its candidate to the one candidate
+// array, so one grid.sync per round serves all models.  After it, each block reduces its own group's candidates to
+// that model's pick and also checks whether any group still has a positive best; when none has, every block leaves.
+// A pick depends only on the model's gains (first index of the largest), never on the block partition, so slice g
+// equals tip_cam_bits on model g.
+__global__ void __launch_bounds__(kCamThreads) cam_bits_stack_kernel(const uint32_t* __restrict__ prof, int n, int words,
+                                                                     int bpm, int32_t* __restrict__ gain,
+                                                                     uint32_t* __restrict__ covered2,
+                                                                     int2* __restrict__ cand2, int32_t* __restrict__ order,
+                                                                     int32_t* __restrict__ state, int max_rounds) {
+  cg::grid_group grid = cg::this_grid();
+  __shared__ int2 s_list[kCamMaxList];
+  __shared__ int s_gain[kCamThreads / 32], s_idx[kCamThreads / 32];
+  __shared__ int s_n, s_pick, s_best;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int nb = gridDim.x;
+  const int g = blockIdx.x / bpm, gb = blockIdx.x - g * bpm, g0 = g * bpm;
+  const int per = (n + bpm - 1) / bpm;
+  const int lo = gb * per, hi = min(n, lo + per);
+  prof += (size_t)g * n * words;
+  gain += (size_t)g * n;
+  covered2 += (size_t)g * 2 * words;
+  order += (size_t)g * n;
+  state += 4 * g;
+  const bool lead = gb == 0 && threadIdx.x == 0;   // records the group's picks and state
+  auto better = [](int a, int i, int a2, int i2) { return a2 > a || (a2 == a && i2 < i); };
+  int picks = state[0];
+  bool done = state[1] != 0;
+  for (int round = 0; round < max_rounds; round++) {
+    const int par = round & 1;
+    // (A) best of the own slice; a finished group publishes (-1, -)
+    int bg = -1, bi = 0x7fffffff;
+    for (int i = lo + threadIdx.x, end = done ? lo : hi; i < end; i += kCamThreads) {
+      const int gi = gain[i];
+      if (gi > bg) { bg = gi; bi = i; }
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+      const int g2 = __shfl_xor_sync(0xffffffffu, bg, o), i2 = __shfl_xor_sync(0xffffffffu, bi, o);
+      if (better(bg, bi, g2, i2)) { bg = g2; bi = i2; }
+    }
+    if (lane == 0) { s_gain[warp] = bg; s_idx[warp] = bi; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      for (int w = 1; w < kCamThreads / 32; w++)
+        if (better(bg, bi, s_gain[w], s_idx[w])) { bg = s_gain[w]; bi = s_idx[w]; }
+      cand2[par * nb + blockIdx.x] = make_int2(bg, bi);
+    }
+    // A finished group keeps taking part in every grid.sync: the barrier counts every block of the grid, so a block
+    // that returned while others still loop would hang it.  Blocks leave only all together, below.
+    grid.sync();
+    // (B) the own model's pick, identically in every block of the group, and whether any group goes on
+    bg = -1; bi = 0x7fffffff;
+    int live = 0;
+    for (int b = threadIdx.x; b < nb; b += kCamThreads) {
+      const int2 c = cand2[par * nb + b];
+      live |= c.x > 0;
+      if (b >= g0 && b < g0 + bpm && better(bg, bi, c.x, c.y)) { bg = c.x; bi = c.y; }
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+      const int g2 = __shfl_xor_sync(0xffffffffu, bg, o), i2 = __shfl_xor_sync(0xffffffffu, bi, o);
+      if (better(bg, bi, g2, i2)) { bg = g2; bi = i2; }
+    }
+    if (lane == 0) { s_gain[warp] = bg; s_idx[warp] = bi; }
+    const bool any_live = __syncthreads_or(live);
+    if (threadIdx.x == 0) {
+      for (int w = 1; w < kCamThreads / 32; w++)
+        if (better(bg, bi, s_gain[w], s_idx[w])) { bg = s_gain[w]; bi = s_idx[w]; }
+      s_best = bg; s_pick = bi; s_n = 0;
+    }
+    __syncthreads();
+    if (!done && s_best <= 0) {                      // nothing new can be covered (prioritizers.py:30-31)
+      done = true;
+      if (lead) { state[1] = 1; state[0] = picks; }
+    }
+    if (!any_live) return;
+    if (done) continue;
+    const int pick = s_pick;
+    const uint32_t* cov = covered2 + (size_t)par * words;
+    uint32_t* cov_next = covered2 + (size_t)(par ^ 1) * words;
+    const uint32_t* prow = prof + (size_t)pick * words;
+    for (int w = threadIdx.x; w < words; w += kCamThreads) {
+      const uint32_t c = cov[w];
+      const uint32_t fresh = prow[w] & ~c;
+      if (gb == 0) cov_next[w] = c | fresh;
+      if (fresh) {
+        const int pos = atomicAdd(&s_n, 1);
+        if (pos < kCamMaxList) s_list[pos] = make_int2(w, (int)fresh);
+      }
+    }
+    __syncthreads();
+    if (lead) order[picks] = pick;
+    picks++;
+    const int nn = s_n;
+    // (C) gains of the own slice
+    for (int i = lo + warp; i < hi; i += kCamThreads / 32) {
+      if (gain[i] == 0) continue;                   // warp-uniform
+      const uint32_t* row = prof + (size_t)i * words;
+      int cnt = 0;
+      if (nn <= kCamMaxList) {
+        for (int e = lane; e < nn; e += 32) cnt += __popc(row[s_list[e].x] & (uint32_t)s_list[e].y);
+      } else {                                      // very dense pick: walk all words
+        for (int w = lane; w < words; w += 32) cnt += __popc(row[w] & prow[w] & ~cov[w]);
+      }
+      cnt = warp_sum(cnt);
+      if (lane == 0 && cnt) gain[i] -= cnt;
+    }
+    __syncthreads();
+  }
+  if (lead) state[0] = picks;
+}
+
 __global__ void __launch_bounds__(256) popcount_rows_kernel(const uint32_t* __restrict__ prof, int n, int words,
                                                             int32_t* __restrict__ gain) {
   const int lane = threadIdx.x & 31;
@@ -465,5 +580,41 @@ extern "C" int tip_cam_bits(const uint32_t* bits, int64_t n, int64_t words, int3
                   (void*)&state, (void*)&mr};
   TIP_CHECK_CUDA(cudaLaunchCooperativeKernel((const void*)cam_bits_kernel, dim3(grid), dim3(kCamThreads), args, 0, st));
   tip::count_launch();
+  return TIP_OK;
+}
+
+extern "C" int tip_cam_bits_stack(const uint32_t* bits, int64_t models, int64_t n, int64_t words, int32_t* gain,
+                                  uint32_t* covered2, int32_t* cand_scratch, int32_t* order, int32_t* state,
+                                  int32_t max_rounds, int32_t init_gain, void* stream) {
+  TIP_REQUIRE(bits && gain && covered2 && cand_scratch && order && state, "null pointer");
+  TIP_REQUIRE(models >= 1 && models < (1LL << 31) && n >= 1 && n < (1LL << 31) && models * n < (1LL << 31) &&
+              words >= 1 && words < (1LL << 31) && max_rounds >= 0, "shape");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (init_gain) {
+    popcount_rows_kernel<<<(unsigned)((models * n + 7) / 8), 256, 0, st>>>(bits, (int)(models * n), (int)words, gain);
+    TIP_LAUNCH_CHECK();
+  }
+  if (max_rounds == 0) return TIP_OK;
+  int per_sm = 0;
+  TIP_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, cam_bits_stack_kernel, kCamThreads, 0));
+  TIP_REQUIRE(per_sm >= 1, "cooperative kernel does not fit");
+  const int cap = (int)std::min<int64_t>((int64_t)sm_count() * std::min(per_sm, 2), TIP_CAM_MAX_BLOCKS);
+  // models beyond one co-resident grid run in consecutive chunks, each model keeping its own state across them
+  for (int64_t m0 = 0; m0 < models; m0 += cap) {
+    const int chunk = (int)std::min<int64_t>(cap, models - m0);
+    int bpm = (int)std::max<int64_t>(1, std::min<int64_t>(cap / chunk, (n + 63) / 64));
+    const uint32_t* b = bits + (size_t)m0 * n * words;
+    int32_t* g = gain + (size_t)m0 * n;
+    uint32_t* cov = covered2 + (size_t)m0 * 2 * words;
+    int32_t* ord = order + (size_t)m0 * n;
+    int32_t* sta = state + (size_t)m0 * 4;
+    int2* cand = (int2*)cand_scratch;
+    int ni = (int)n, wi = (int)words, mr = max_rounds;
+    void* args[] = {(void*)&b, (void*)&ni, (void*)&wi, (void*)&bpm, (void*)&g, (void*)&cov, (void*)&cand,
+                    (void*)&ord, (void*)&sta, (void*)&mr};
+    TIP_CHECK_CUDA(cudaLaunchCooperativeKernel((const void*)cam_bits_stack_kernel, dim3(chunk * bpm), dim3(kCamThreads),
+                                               args, 0, st));
+    tip::count_launch();
+  }
   return TIP_OK;
 }
