@@ -8,7 +8,7 @@ device and nothing is written to disk.
 """
 from __future__ import annotations
 
-from typing import Callable, Dict, List, Sequence, Tuple
+from typing import Dict, List, Sequence, Tuple
 
 import numpy as np
 
@@ -17,6 +17,24 @@ from .aggregate_statistics import AggregateStatisticsCollector
 from .neuron_coverage import KMNC, NAC, NBC, SNAC, TKNC, CoverageMethod, _score_dtype
 from .prioritizers import cam_from_bits, cam_from_bits_stack
 from .timer import Timer
+
+# The study's twelve coverage metrics (handler_coverage.py:49-101) as (id, debit, factory): the factory builds the
+# metric from one model's per-layer mins, maxs and stds, and the debit names its share of the training walk
+# (`_walk_debits`).  A debit of None marks a metric built from no training statistics: it is charged nothing and
+# holds no state, so one object serves every model of a stack.
+METRICS = (
+    [(f"NBC_{s}", "NBC", lambda mn, mx, sd, s=s: NBC(mins=mn, maxs=mx, stds=sd, scaler=s)) for s in (0, 0.5, 1)]
+    + [(f"SNAC_{s}", "SNAC", lambda mn, mx, sd, s=s: SNAC(maxs=mx, stds=sd, scaler=s)) for s in (0, 0.5, 1)]
+    + [("NAC_0", None, lambda *_: NAC(cov_threshold=0.0)), ("NAC_0.75", None, lambda *_: NAC(cov_threshold=0.75))]
+    + [(f"TKNC_{k}", None, lambda *_, k=k: TKNC(top_neurons=k)) for k in (1, 2, 3)]
+    + [("KMNC_2", "KMNC", lambda mn, mx, sd: KMNC(mn, mx, sections=2))])
+
+
+def _walk_debits(agg_stats: AggregateStatisticsCollector, pred_timer: Timer) -> Dict:
+    """The debits of `METRICS` in seconds; the collector books min, max and Welford on its welford timer."""
+    mn, mx, wf = agg_stats.min_timer.get(), agg_stats.max_timer.get(), agg_stats.welford_timer.get()
+    pred = pred_timer.get()
+    return {"NBC": mn + mx + pred + wf, "SNAC": wf + mx + pred, "KMNC": mn + mx + pred, None: 0.0}
 
 
 class CoverageWorker(HookedModelHandler):
@@ -56,24 +74,11 @@ class CoverageWorker(HookedModelHandler):
         mins, maxs, std = agg_stats.get()
         self.mins, self.maxs, self.stds = mins, maxs, std          # per layer, layer-shaped
 
-        # handler_coverage.py:49-101; the collector books min, max and Welford on its welford timer
-        nbc_debit = agg_stats.min_timer.get() + agg_stats.max_timer.get() + pred_timer.get() + agg_stats.welford_timer.get()
-        for s in (0, 0.5, 1):
-            self._add_metric(f"NBC_{s}", lambda s=s: NBC(mins=mins, maxs=maxs, stds=std, scaler=s), nbc_debit)
-        snac_debit = agg_stats.welford_timer.get() + agg_stats.max_timer.get() + pred_timer.get()
-        for s in (0, 0.5, 1):
-            self._add_metric(f"SNAC_{s}", lambda s=s: SNAC(maxs=maxs, stds=std, scaler=s), snac_debit)
-        self._add_metric("NAC_0", lambda: NAC(cov_threshold=0.0))
-        self._add_metric("NAC_0.75", lambda: NAC(cov_threshold=0.75))
-        for k in (1, 2, 3):
-            self._add_metric(f"TKNC_{k}", lambda k=k: TKNC(top_neurons=k))
-        kmnc_debit = agg_stats.min_timer.get() + agg_stats.max_timer.get() + pred_timer.get()
-        self._add_metric("KMNC_2", lambda: KMNC(mins, maxs, sections=2), kmnc_debit)
-
-    def _add_metric(self, metric_id: str, metric_supplier: Callable[[], CoverageMethod], time_debit: float = 0.0):
-        timer = Timer()
-        self.metrics[metric_id] = self._synced(metric_supplier, timer)
-        self.setup_times[metric_id] = time_debit + timer.get()
+        debits = _walk_debits(agg_stats, pred_timer)
+        for metric_id, debit, factory in METRICS:
+            timer = Timer()
+            self.metrics[metric_id] = self._synced(lambda: factory(mins, maxs, std), timer)
+            self.setup_times[metric_id] = debits[debit] + timer.get()
 
     def _traces(self, data) -> Tuple[List, object]:
         """The test set's hooked layers on the scoring device (moved there once if the model lives elsewhere), and
@@ -183,30 +188,18 @@ class StackedCoverageWorker(HookedModelHandler):
         m_range = range(self.models)
         self.mins, self.maxs, self.stds = ([[layer[m] for layer in stat] for m in m_range] for stat in (mins, maxs, std))
 
-        nbc_debit = agg_stats.min_timer.get() + agg_stats.max_timer.get() + pred_timer.get() + agg_stats.welford_timer.get()
-        for s in (0, 0.5, 1):
-            self._add_metric(f"NBC_{s}", lambda s=s: [NBC(mins=self.mins[m], maxs=self.maxs[m], stds=self.stds[m],
-                                                          scaler=s) for m in m_range], nbc_debit)
-        snac_debit = agg_stats.welford_timer.get() + agg_stats.max_timer.get() + pred_timer.get()
-        for s in (0, 0.5, 1):
-            self._add_metric(f"SNAC_{s}", lambda s=s: [SNAC(maxs=self.maxs[m], stds=self.stds[m], scaler=s)
-                                                       for m in m_range], snac_debit)
-        self._add_metric("NAC_0", lambda: [NAC(cov_threshold=0.0)])
-        self._add_metric("NAC_0.75", lambda: [NAC(cov_threshold=0.75)])
-        for k in (1, 2, 3):
-            self._add_metric(f"TKNC_{k}", lambda k=k: [TKNC(top_neurons=k)])
-        kmnc_debit = agg_stats.min_timer.get() + agg_stats.max_timer.get() + pred_timer.get()
-        self._add_metric("KMNC_2", lambda: [KMNC(self.mins[m], self.maxs[m], sections=2) for m in m_range], kmnc_debit)
+        debits = _walk_debits(agg_stats, pred_timer)
+        for metric_id, debit, factory in METRICS:
+            timer = Timer()
+            built = range(1) if debit is None else m_range        # a stateless metric: one object for all M models
+            self.metrics[metric_id] = self._synced(
+                lambda: [factory(self.mins[m], self.maxs[m], self.stds[m]) for m in built], timer)
+            self.setup_times[metric_id] = (debits[debit] + timer.get()) / self.models
 
     def _activations(self, badge):
         """The hooked layers of one stacked forward on `badge` (every model sees it), each [M, b, *layer shape]."""
         acts = self.base_model.get_activations(self.stack.stack_inputs([badge] * self.models))
         return [self.stack.model_major(child, a) for child, a in zip(self.nc_layers, acts)]
-
-    def _add_metric(self, metric_id: str, metric_supplier: Callable[[], List[CoverageMethod]], time_debit: float = 0.0):
-        timer = Timer()
-        self.metrics[metric_id] = self._synced(metric_supplier, timer)
-        self.setup_times[metric_id] = (time_debit + timer.get()) / self.models
 
     def _traces(self, data):
         """The test set's traces as one model-major [M, N, D] tensor on the scoring device (each model's layers

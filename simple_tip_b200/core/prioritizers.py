@@ -39,44 +39,55 @@ def _tail_by_score(scores: np.ndarray, greedy: np.ndarray):
         yield int(i)
 
 
-def cam_from_bits(scores: np.ndarray, bits, rounds_per_launch: int = 4096) -> Generator[int, None, None]:
-    """`cam(scores, profiles)` for a boolean profile given bit-packed in HBM: bits [N, words] int32 CUDA
-    tensor (any consistent packing — `NAC/NBC/SNAC/TKNC.packed()` or `pack_profiles`).  The greedy loop
-    (prioritizers.py:24-45) is ONE persistent cooperative kernel (libb200tip `tip_cam_bits`): per round an
-    arg-max of the gains, new = profile[pick] & ~covered, gain -= popcount(profile & new)."""
+def _greedy_bits(bits, rounds_per_launch: int, stack: bool):
+    """The greedy picks of M profiles, bits [M, N, words] int32 CUDA tensor with N, words >= 1, and the device time
+    of the loop in ms (CUDA events around the launches).  The loop is libb200tip `tip_cam_bits_stack`, or
+    `tip_cam_bits` when not `stack` (M = 1), launched until no model is still live (not done and fewer than N
+    picks), `rounds_per_launch` rounds per launch.  Returns (M int64 pick arrays, ms)."""
     import torch
 
     from .. import _lib
     from .. import engine as E
 
+    lib = _lib.load()
+    models, n, words = (int(s) for s in bits.shape)
+    entry, dims = ("tip_cam_bits_stack", (models, n, words)) if stack else ("tip_cam_bits", (n, words))
+    dev = bits.device
+    bits = bits.contiguous()
+    gain = torch.empty((models, n), dtype=torch.int32, device=dev)
+    covered = torch.zeros((models, 2 * words), dtype=torch.int32, device=dev)
+    cand = torch.zeros(4 * _lib.CAM_MAX_BLOCKS, dtype=torch.int32, device=dev)
+    order = torch.zeros((models, n), dtype=torch.int32, device=dev)
+    state = torch.zeros((models, 4), dtype=torch.int32, device=dev)
+    rounds = max(2, int(rounds_per_launch) & ~1)              # even: the covered sets are double-buffered by parity
+    first = 1
+    ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    ev0.record()
+    while True:
+        _lib.check(getattr(lib, entry)(E._p(bits), *dims, E._p(gain), E._p(covered), E._p(cand), E._p(order),
+                                       E._p(state), rounds, first, E._stream()), entry)
+        first = 0
+        ev1.record()
+        st = state.cpu().numpy()
+        if not np.any((st[:, 1] == 0) & (st[:, 0] < n)):
+            break
+    picked = order[:, :int(st[:, 0].max())].cpu().numpy()
+    return [picked[m, :st[m, 0]].astype(np.int64) for m in range(models)], float(ev0.elapsed_time(ev1))
+
+
+def cam_from_bits(scores: np.ndarray, bits, rounds_per_launch: int = 4096) -> Generator[int, None, None]:
+    """`cam(scores, profiles)` for a boolean profile given bit-packed in HBM: bits [N, words] int32 CUDA
+    tensor (any consistent packing — `NAC/NBC/SNAC/TKNC.packed()` or `pack_profiles`).  The greedy loop
+    (prioritizers.py:24-45) is ONE persistent cooperative kernel (libb200tip `tip_cam_bits`): per round an
+    arg-max of the gains, new = profile[pick] & ~covered, gain -= popcount(profile & new)."""
     scores = np.asarray(scores).copy()
     assert scores.ndim == 1
-    lib = _lib.load()
     n, words = int(bits.shape[0]), int(bits.shape[1]) if bits.ndim == 2 else 0
     assert scores.shape[0] == n, "one score per sample"
     greedy = np.zeros(0, dtype=np.int64)
     if n > 0 and words > 0:
-        dev = bits.device
-        bits = bits.contiguous()
-        gain = torch.empty(n, dtype=torch.int32, device=dev)
-        covered = torch.zeros(2 * words, dtype=torch.int32, device=dev)
-        cand = torch.zeros(4 * _lib.CAM_MAX_BLOCKS, dtype=torch.int32, device=dev)
-        order = torch.zeros(n, dtype=torch.int32, device=dev)
-        state = torch.zeros(4, dtype=torch.int32, device=dev)
-        picks, done, first = 0, False, 1
-        rounds = max(2, int(rounds_per_launch) & ~1)              # even: the covered set is double-buffered by parity
-        ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        ev0.record()
-        while not done and picks < n:
-            _lib.check(lib.tip_cam_bits(E._p(bits), n, words, E._p(gain), E._p(covered), E._p(cand), E._p(order),
-                                        E._p(state), rounds, first, E._stream()), "tip_cam_bits")
-            first = 0
-            ev1.record()
-            st = state.cpu().numpy()
-            picks, done = int(st[0]), bool(st[1])
-        greedy = order[:picks].cpu().numpy().astype(np.int64)
         global LAST_GREEDY_MS
-        LAST_GREEDY_MS = float(ev0.elapsed_time(ev1))
+        (greedy,), LAST_GREEDY_MS = _greedy_bits(bits[None], rounds_per_launch, stack=False)
     global LAST_GREEDY_PICKS
     LAST_GREEDY_PICKS = int(greedy.shape[0])
     yield from (int(i) for i in greedy)
@@ -89,37 +100,13 @@ def cam_from_bits_stack(scores: Sequence[np.ndarray], bits, rounds_per_launch: i
     `tip_cam_bits_stack`), one grid barrier per round for all of them; each model's remaining samples then follow
     by its scores on the host (`_tail_by_score`).  Returns, per model m, the int64 order
     `list(cam_from_bits(scores[m], bits[m]))` gives."""
-    import torch
-
-    from .. import _lib
-    from .. import engine as E
-
     scores = [np.asarray(s).copy() for s in scores]
     assert bits.ndim == 3, "bits [M, N, words]"
     models, n, words = (int(s) for s in bits.shape)
     assert len(scores) == models and all(s.ndim == 1 and s.shape[0] == n for s in scores), "M vectors of N scores"
     greedy = [np.zeros(0, dtype=np.int64)] * models
     if models > 0 and n > 0 and words > 0:
-        lib = _lib.load()
-        dev = bits.device
-        bits = bits.contiguous()
-        gain = torch.empty((models, n), dtype=torch.int32, device=dev)
-        covered = torch.zeros((models, 2 * words), dtype=torch.int32, device=dev)
-        cand = torch.zeros(4 * _lib.CAM_MAX_BLOCKS, dtype=torch.int32, device=dev)
-        order = torch.zeros((models, n), dtype=torch.int32, device=dev)
-        state = torch.zeros((models, 4), dtype=torch.int32, device=dev)
-        rounds = max(2, int(rounds_per_launch) & ~1)              # even: the covered sets are double-buffered by parity
-        first = 1
-        while True:
-            _lib.check(lib.tip_cam_bits_stack(E._p(bits), models, n, words, E._p(gain), E._p(covered), E._p(cand),
-                                              E._p(order), E._p(state), rounds, first, E._stream()),
-                       "tip_cam_bits_stack")
-            first = 0
-            st = state.cpu().numpy()
-            if not np.any((st[:, 1] == 0) & (st[:, 0] < n)):
-                break
-        picked = order.cpu().numpy()
-        greedy = [picked[m, :st[m, 0]].astype(np.int64) for m in range(models)]
+        greedy, _ = _greedy_bits(bits, rounds_per_launch, stack=True)
     return [np.fromiter(itertools.chain(g, _tail_by_score(s, g)), dtype=np.int64) for s, g in zip(scores, greedy)]
 
 

@@ -13,8 +13,8 @@
 //                        applied sample by sample in the activation dtype — reproduced bit for bit)
 //   tip_cam_bits         cam() of prioritizers.py:16-45 on bit-packed profiles, one persistent
 //                        cooperative kernel for all greedy rounds
-//   tip_cam_bits_stack   the same for the profiles of a stack of models: one greedy loop per model, all under one
-//                        grid barrier per round
+//   tip_cam_bits_stack   the same kernel's STACK instance for the profiles of a stack of models: one greedy loop
+//                        per model, all under one grid barrier per round
 //
 // All three profile kernels write the reference's dense boolean profile (one byte per entry, what the
 // classes return) and/or the same profile bit-packed for tip_cam_bits.  Packed layout (a fixed
@@ -230,131 +230,55 @@ __global__ void __launch_bounds__(128) stats_update_kernel(const T* __restrict__
 // set; (C) every block subtracts popcount(profile[n] & new) from the gains of its slice.  A block only ever
 // reads gains it wrote itself, so one grid.sync per round suffices (candidates and covered are
 // double-buffered by round parity).
+//
+// STACK: the profiles of a stack of models, one greedy loop per model under the same grid.sync.  The grid is cut
+// into gridDim.x / bpm groups of bpm consecutive blocks; group g runs (A)/(B)/(C) on model g's profile, gains,
+// covered set, order and state, and its first block takes block 0's part.  After the barrier each block reduces
+// its own group's candidates to that model's pick and also checks whether any group still has a positive best;
+// when none has, every block leaves.  A pick depends only on the model's gains (first index of the largest), never
+// on the block partition, so slice g equals the single-model kernel on model g.  bpm is a parameter of the stack
+// instance only (the pack Bpm is empty for STACK = false), so each instance keeps its own parameter layout.
 constexpr int kCamThreads = 256;
 constexpr int kCamMaxList = 4096;     // non-zero words of `new` kept in shared memory (32 KB as int2)
 
+template <bool STACK, class... Bpm>
 __global__ void __launch_bounds__(kCamThreads) cam_bits_kernel(const uint32_t* __restrict__ prof, int n, int words,
-                                                               int32_t* __restrict__ gain, uint32_t* __restrict__ covered2,
+                                                               Bpm... bpm_arg, int32_t* __restrict__ gain,
+                                                               uint32_t* __restrict__ covered2,
                                                                int2* __restrict__ cand2, int32_t* __restrict__ order,
                                                                int32_t* __restrict__ state, int max_rounds) {
+  static_assert(sizeof...(Bpm) == (STACK ? 1 : 0), "bpm (blocks per model) is the stack instance's parameter");
   cg::grid_group grid = cg::this_grid();
   __shared__ int2 s_list[kCamMaxList];
   __shared__ int s_gain[kCamThreads / 32], s_idx[kCamThreads / 32];
   __shared__ int s_n, s_pick, s_best;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int nb = gridDim.x;
-  const int per = (n + nb - 1) / nb;
-  const int lo = blockIdx.x * per, hi = min(n, lo + per);
-  auto better = [](int g, int i, int g2, int i2) { return g2 > g || (g2 == g && i2 < i); };
-  int picks = state[0];
-  if (state[1]) return;
-  for (int round = 0; round < max_rounds; round++) {
-    const int par = round & 1;
-    // (A) best of the own slice
-    int bg = -1, bi = 0x7fffffff;
-    for (int i = lo + threadIdx.x; i < hi; i += kCamThreads) {
-      const int g = gain[i];
-      if (g > bg) { bg = g; bi = i; }
-    }
-    for (int o = 16; o > 0; o >>= 1) {
-      const int g2 = __shfl_xor_sync(0xffffffffu, bg, o), i2 = __shfl_xor_sync(0xffffffffu, bi, o);
-      if (better(bg, bi, g2, i2)) { bg = g2; bi = i2; }
-    }
-    if (lane == 0) { s_gain[warp] = bg; s_idx[warp] = bi; }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      for (int w = 1; w < kCamThreads / 32; w++)
-        if (better(bg, bi, s_gain[w], s_idx[w])) { bg = s_gain[w]; bi = s_idx[w]; }
-      cand2[par * nb + blockIdx.x] = make_int2(bg, bi);
-    }
-    grid.sync();
-    // (B) the pick, identically in every block
-    bg = -1; bi = 0x7fffffff;
-    for (int b = threadIdx.x; b < nb; b += kCamThreads) {
-      const int2 c = cand2[par * nb + b];
-      if (better(bg, bi, c.x, c.y)) { bg = c.x; bi = c.y; }
-    }
-    for (int o = 16; o > 0; o >>= 1) {
-      const int g2 = __shfl_xor_sync(0xffffffffu, bg, o), i2 = __shfl_xor_sync(0xffffffffu, bi, o);
-      if (better(bg, bi, g2, i2)) { bg = g2; bi = i2; }
-    }
-    if (lane == 0) { s_gain[warp] = bg; s_idx[warp] = bi; }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      for (int w = 1; w < kCamThreads / 32; w++)
-        if (better(bg, bi, s_gain[w], s_idx[w])) { bg = s_gain[w]; bi = s_idx[w]; }
-      s_best = bg; s_pick = bi; s_n = 0;
-    }
-    __syncthreads();
-    if (s_best <= 0) {                               // nothing new can be covered (prioritizers.py:30-31)
-      if (blockIdx.x == 0 && threadIdx.x == 0) { state[1] = 1; state[0] = picks; }
-      return;
-    }
-    const int pick = s_pick;
-    const uint32_t* cov = covered2 + (size_t)par * words;
-    uint32_t* cov_next = covered2 + (size_t)(par ^ 1) * words;
-    const uint32_t* prow = prof + (size_t)pick * words;
-    for (int w = threadIdx.x; w < words; w += kCamThreads) {
-      const uint32_t c = cov[w];
-      const uint32_t fresh = prow[w] & ~c;
-      if (blockIdx.x == 0) cov_next[w] = c | fresh;
-      if (fresh) {
-        const int pos = atomicAdd(&s_n, 1);
-        if (pos < kCamMaxList) s_list[pos] = make_int2(w, (int)fresh);
-      }
-    }
-    __syncthreads();
-    if (blockIdx.x == 0 && threadIdx.x == 0) order[picks] = pick;
-    picks++;
-    const int nn = s_n;
-    // (C) gains of the own slice
-    for (int i = lo + warp; i < hi; i += kCamThreads / 32) {
-      if (gain[i] == 0) continue;                   // warp-uniform
-      const uint32_t* row = prof + (size_t)i * words;
-      int cnt = 0;
-      if (nn <= kCamMaxList) {
-        for (int e = lane; e < nn; e += 32) cnt += __popc(row[s_list[e].x] & (uint32_t)s_list[e].y);
-      } else {                                      // very dense pick: walk all words
-        for (int w = lane; w < words; w += 32) cnt += __popc(row[w] & prow[w] & ~cov[w]);
-      }
-      cnt = warp_sum(cnt);
-      if (lane == 0 && cnt) gain[i] -= cnt;
-    }
-    __syncthreads();
+  int bpm = nb, g = 0, gb = blockIdx.x;            // one model: one group of all blocks
+  if constexpr (STACK) {
+    bpm = (bpm_arg + ...);
+    g = blockIdx.x / bpm;
+    gb = blockIdx.x - g * bpm;
   }
-  if (blockIdx.x == 0 && threadIdx.x == 0) state[0] = picks;
-}
-
-// ---- CAM for a stack of models: independent greedy loops under one grid barrier per round ----------------------------
-// The grid is cut into gridDim.x / bpm groups of bpm consecutive blocks; group g runs cam_bits_kernel's (A)/(B)/(C) on
-// model g's profile, gains, covered set, order and state.  Every block publishes its candidate to the one candidate
-// array, so one grid.sync per round serves all models.  After it, each block reduces its own group's candidates to
-// that model's pick and also checks whether any group still has a positive best; when none has, every block leaves.
-// A pick depends only on the model's gains (first index of the largest), never on the block partition, so slice g
-// equals tip_cam_bits on model g.
-__global__ void __launch_bounds__(kCamThreads) cam_bits_stack_kernel(const uint32_t* __restrict__ prof, int n, int words,
-                                                                     int bpm, int32_t* __restrict__ gain,
-                                                                     uint32_t* __restrict__ covered2,
-                                                                     int2* __restrict__ cand2, int32_t* __restrict__ order,
-                                                                     int32_t* __restrict__ state, int max_rounds) {
-  cg::grid_group grid = cg::this_grid();
-  __shared__ int2 s_list[kCamMaxList];
-  __shared__ int s_gain[kCamThreads / 32], s_idx[kCamThreads / 32];
-  __shared__ int s_n, s_pick, s_best;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int nb = gridDim.x;
-  const int g = blockIdx.x / bpm, gb = blockIdx.x - g * bpm, g0 = g * bpm;
+  const int g0 = g * bpm;
   const int per = (n + bpm - 1) / bpm;
   const int lo = gb * per, hi = min(n, lo + per);
-  prof += (size_t)g * n * words;
-  gain += (size_t)g * n;
-  covered2 += (size_t)g * 2 * words;
-  order += (size_t)g * n;
-  state += 4 * g;
-  const bool lead = gb == 0 && threadIdx.x == 0;   // records the group's picks and state
+  if constexpr (STACK) {
+    prof += (size_t)g * n * words;
+    gain += (size_t)g * n;
+    covered2 += (size_t)g * 2 * words;
+    order += (size_t)g * n;
+    state += 4 * g;
+  }
+  // the thread that records the group's picks and state; the single-model instance tests it at each store, as
+  // hoisting the test would change that instance's code
+  const bool first_thread = gb == 0 && threadIdx.x == 0;
+  auto lead = [&] { return STACK ? first_thread : gb == 0 && threadIdx.x == 0; };
   auto better = [](int a, int i, int a2, int i2) { return a2 > a || (a2 == a && i2 < i); };
   int picks = state[0];
-  bool done = state[1] != 0;
+  bool done = false;
+  if constexpr (STACK) done = state[1] != 0;      // a finished group still joins every grid.sync, see below
+  else if (state[1]) return;
   for (int round = 0; round < max_rounds; round++) {
     const int par = round & 1;
     // (A) best of the own slice; a finished group publishes (-1, -)
@@ -374,8 +298,8 @@ __global__ void __launch_bounds__(kCamThreads) cam_bits_stack_kernel(const uint3
         if (better(bg, bi, s_gain[w], s_idx[w])) { bg = s_gain[w]; bi = s_idx[w]; }
       cand2[par * nb + blockIdx.x] = make_int2(bg, bi);
     }
-    // A finished group keeps taking part in every grid.sync: the barrier counts every block of the grid, so a block
-    // that returned while others still loop would hang it.  Blocks leave only all together, below.
+    // STACK: a finished group keeps taking part in every grid.sync: the barrier counts every block of the grid, so a
+    // block that returned while others still loop would hang it.  Blocks leave only all together, below.
     grid.sync();
     // (B) the own model's pick, identically in every block of the group, and whether any group goes on
     bg = -1; bi = 0x7fffffff;
@@ -383,14 +307,16 @@ __global__ void __launch_bounds__(kCamThreads) cam_bits_stack_kernel(const uint3
     for (int b = threadIdx.x; b < nb; b += kCamThreads) {
       const int2 c = cand2[par * nb + b];
       live |= c.x > 0;
-      if (b >= g0 && b < g0 + bpm && better(bg, bi, c.x, c.y)) { bg = c.x; bi = c.y; }
+      if ((!STACK || (b >= g0 && b < g0 + bpm)) && better(bg, bi, c.x, c.y)) { bg = c.x; bi = c.y; }
     }
     for (int o = 16; o > 0; o >>= 1) {
       const int g2 = __shfl_xor_sync(0xffffffffu, bg, o), i2 = __shfl_xor_sync(0xffffffffu, bi, o);
       if (better(bg, bi, g2, i2)) { bg = g2; bi = i2; }
     }
     if (lane == 0) { s_gain[warp] = bg; s_idx[warp] = bi; }
-    const bool any_live = __syncthreads_or(live);
+    bool any_live = true;
+    if constexpr (STACK) any_live = __syncthreads_or(live);
+    else __syncthreads();
     if (threadIdx.x == 0) {
       for (int w = 1; w < kCamThreads / 32; w++)
         if (better(bg, bi, s_gain[w], s_idx[w])) { bg = s_gain[w]; bi = s_idx[w]; }
@@ -399,7 +325,8 @@ __global__ void __launch_bounds__(kCamThreads) cam_bits_stack_kernel(const uint3
     __syncthreads();
     if (!done && s_best <= 0) {                      // nothing new can be covered (prioritizers.py:30-31)
       done = true;
-      if (lead) { state[1] = 1; state[0] = picks; }
+      if (lead()) { state[1] = 1; state[0] = picks; }
+      if constexpr (!STACK) return;
     }
     if (!any_live) return;
     if (done) continue;
@@ -417,7 +344,7 @@ __global__ void __launch_bounds__(kCamThreads) cam_bits_stack_kernel(const uint3
       }
     }
     __syncthreads();
-    if (lead) order[picks] = pick;
+    if (lead()) order[picks] = pick;
     picks++;
     const int nn = s_n;
     // (C) gains of the own slice
@@ -435,7 +362,7 @@ __global__ void __launch_bounds__(kCamThreads) cam_bits_stack_kernel(const uint3
     }
     __syncthreads();
   }
-  if (lead) state[0] = picks;
+  if (lead()) state[0] = picks;
 }
 
 __global__ void __launch_bounds__(256) popcount_rows_kernel(const uint32_t* __restrict__ prof, int n, int words,
@@ -558,48 +485,26 @@ extern "C" int tip_pack_bool(const void* profile_u8, int64_t n, int64_t f, uint3
   return TIP_OK;
 }
 
-extern "C" int tip_cam_bits(const uint32_t* bits, int64_t n, int64_t words, int32_t* gain, uint32_t* covered2,
-                            int32_t* cand_scratch, int32_t* order, int32_t* state, int32_t max_rounds, int32_t init_gain,
-                            void* stream) {
-  TIP_REQUIRE(bits && gain && covered2 && cand_scratch && order && state, "null pointer");
-  TIP_REQUIRE(n >= 1 && n < (1LL << 31) && words >= 1 && words < (1LL << 31) && max_rounds >= 0, "shape");
-  cudaStream_t st = (cudaStream_t)stream;
-  if (init_gain) {
-    popcount_rows_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(bits, (int)n, (int)words, gain);
-    TIP_LAUNCH_CHECK();
-  }
-  if (max_rounds == 0) return TIP_OK;
-  int per_sm = 0;
-  TIP_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, cam_bits_kernel, kCamThreads, 0));
-  TIP_REQUIRE(per_sm >= 1, "cooperative kernel does not fit");
-  int grid = std::min<int64_t>((int64_t)sm_count() * std::min(per_sm, 2), (n + 63) / 64);
-  grid = std::max(1, std::min(grid, TIP_CAM_MAX_BLOCKS));
-  int ni = (int)n, wi = (int)words, mr = max_rounds;
-  int2* cand = (int2*)cand_scratch;
-  void* args[] = {(void*)&bits, (void*)&ni, (void*)&wi, (void*)&gain, (void*)&covered2, (void*)&cand, (void*)&order,
-                  (void*)&state, (void*)&mr};
-  TIP_CHECK_CUDA(cudaLaunchCooperativeKernel((const void*)cam_bits_kernel, dim3(grid), dim3(kCamThreads), args, 0, st));
-  tip::count_launch();
-  return TIP_OK;
-}
-
-extern "C" int tip_cam_bits_stack(const uint32_t* bits, int64_t models, int64_t n, int64_t words, int32_t* gain,
-                                  uint32_t* covered2, int32_t* cand_scratch, int32_t* order, int32_t* state,
-                                  int32_t max_rounds, int32_t init_gain, void* stream) {
-  TIP_REQUIRE(bits && gain && covered2 && cand_scratch && order && state, "null pointer");
-  TIP_REQUIRE(models >= 1 && models < (1LL << 31) && n >= 1 && n < (1LL << 31) && models * n < (1LL << 31) &&
-              words >= 1 && words < (1LL << 31) && max_rounds >= 0, "shape");
+// Both CAM entry points: `models` profiles [n, words] back to back, each with its own gains, covered set, order and
+// state.  A co-resident grid holds cap blocks; a chunk of c models gets bpm = max(1, min(cap / c, ceil(n / 64)))
+// blocks per model.  For one model (tip_cam_bits) that is one group of max(1, min(SMs x min(per_sm, 2), ceil(n / 64),
+// TIP_CAM_MAX_BLOCKS)) blocks: at most two per SM and at least 64 samples per block.  Models beyond one co-resident
+// grid run in consecutive chunks, each model keeping its own state across them.
+template <bool STACK>
+static int cam_bits_launch(const uint32_t* bits, int64_t models, int64_t n, int64_t words, int32_t* gain,
+                           uint32_t* covered2, int32_t* cand_scratch, int32_t* order, int32_t* state, int32_t max_rounds,
+                           int32_t init_gain, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   if (init_gain) {
     popcount_rows_kernel<<<(unsigned)((models * n + 7) / 8), 256, 0, st>>>(bits, (int)(models * n), (int)words, gain);
     TIP_LAUNCH_CHECK();
   }
   if (max_rounds == 0) return TIP_OK;
+  const void* kernel = STACK ? (const void*)cam_bits_kernel<true, int> : (const void*)cam_bits_kernel<false>;
   int per_sm = 0;
-  TIP_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, cam_bits_stack_kernel, kCamThreads, 0));
+  TIP_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kCamThreads, 0));
   TIP_REQUIRE(per_sm >= 1, "cooperative kernel does not fit");
   const int cap = (int)std::min<int64_t>((int64_t)sm_count() * std::min(per_sm, 2), TIP_CAM_MAX_BLOCKS);
-  // models beyond one co-resident grid run in consecutive chunks, each model keeping its own state across them
   for (int64_t m0 = 0; m0 < models; m0 += cap) {
     const int chunk = (int)std::min<int64_t>(cap, models - m0);
     int bpm = (int)std::max<int64_t>(1, std::min<int64_t>(cap / chunk, (n + 63) / 64));
@@ -612,9 +517,30 @@ extern "C" int tip_cam_bits_stack(const uint32_t* bits, int64_t models, int64_t 
     int ni = (int)n, wi = (int)words, mr = max_rounds;
     void* args[] = {(void*)&b, (void*)&ni, (void*)&wi, (void*)&bpm, (void*)&g, (void*)&cov, (void*)&cand,
                     (void*)&ord, (void*)&sta, (void*)&mr};
-    TIP_CHECK_CUDA(cudaLaunchCooperativeKernel((const void*)cam_bits_stack_kernel, dim3(chunk * bpm), dim3(kCamThreads),
-                                               args, 0, st));
+    void* args_one[] = {(void*)&b, (void*)&ni, (void*)&wi, (void*)&g, (void*)&cov, (void*)&cand, (void*)&ord,
+                        (void*)&sta, (void*)&mr};   // cam_bits_kernel<false> takes no bpm
+    TIP_CHECK_CUDA(cudaLaunchCooperativeKernel(kernel, dim3(chunk * bpm), dim3(kCamThreads), STACK ? args : args_one,
+                                               0, st));
     tip::count_launch();
   }
   return TIP_OK;
+}
+
+extern "C" int tip_cam_bits(const uint32_t* bits, int64_t n, int64_t words, int32_t* gain, uint32_t* covered2,
+                            int32_t* cand_scratch, int32_t* order, int32_t* state, int32_t max_rounds, int32_t init_gain,
+                            void* stream) {
+  TIP_REQUIRE(bits && gain && covered2 && cand_scratch && order && state, "null pointer");
+  TIP_REQUIRE(n >= 1 && n < (1LL << 31) && words >= 1 && words < (1LL << 31) && max_rounds >= 0, "shape");
+  return cam_bits_launch<false>(bits, 1, n, words, gain, covered2, cand_scratch, order, state, max_rounds, init_gain,
+                                stream);
+}
+
+extern "C" int tip_cam_bits_stack(const uint32_t* bits, int64_t models, int64_t n, int64_t words, int32_t* gain,
+                                  uint32_t* covered2, int32_t* cand_scratch, int32_t* order, int32_t* state,
+                                  int32_t max_rounds, int32_t init_gain, void* stream) {
+  TIP_REQUIRE(bits && gain && covered2 && cand_scratch && order && state, "null pointer");
+  TIP_REQUIRE(models >= 1 && models < (1LL << 31) && n >= 1 && n < (1LL << 31) && models * n < (1LL << 31) &&
+              words >= 1 && words < (1LL << 31) && max_rounds >= 0, "shape");
+  return cam_bits_launch<true>(bits, models, n, words, gain, covered2, cand_scratch, order, state, max_rounds,
+                               init_gain, stream);
 }
