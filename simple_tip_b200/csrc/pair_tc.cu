@@ -782,24 +782,31 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             atomicOr(reinterpret_cast<unsigned long long*>(args.timeline) + (int64_t)(tl_tile0 + t) * 16 + 3,
                      1ull << cw);
           if (any) {
+            // rare: the tile runs past the span, or some row of the warp must ignore train rows inside it.  One
+            // warp-uniform test per tile, so a full tile without excluded rows pays no per-chunk branch.
+            bool masked = partial;
+            if (EXCL)
+              masked = __any_sync(0xffffffffu, partial || (col_base < st[0].ex_hi && col_base + BN > st[0].ex_lo) ||
+                                                    (col_base < st[1].ex_hi && col_base + BN > st[1].ex_lo));
+            if (masked) {
 #pragma unroll
-            for (int h = 0; h < 2; h++)
+              for (int h = 0; h < 2; h++)
 #pragma unroll
-              for (int c = 0; c < kEvSlots; c++) {
-                const int cbase = col_base + 32 * c;
-                if (partial || (EXCL && cbase < st[h].ex_hi && cbase + 32 > st[h].ex_lo)) {
-                  // rare: the chunk runs past the span, or overlaps the train rows this query must ignore.  The
-                  // accumulator is free to overwrite: the next tile's first MMA does not accumulate.
-                  float mn = kInf;
+                for (int c = 0; c < kEvSlots; c++) {
+                  const int cbase = col_base + 32 * c;
+                  if (partial || (EXCL && cbase < st[h].ex_hi && cbase + 32 > st[h].ex_lo)) {
+                    // The accumulator is free to overwrite: the next tile's first MMA does not accumulate.
+                    float mn = kInf;
 #pragma unroll
-                  for (int k = 0; k < 8; k++) {
-                    const int col = cbase + 8 * (k >> 1) + 2 * sub + (k & 1);
-                    if (col >= st[h].col1 || (EXCL && col >= st[h].ex_lo && col < st[h].ex_hi)) a[ai(h, c, k)] = kInf;
-                    mn = fminf(mn, a[ai(h, c, k)]);
+                    for (int k = 0; k < 8; k++) {
+                      const int col = cbase + 8 * (k >> 1) + 2 * sub + (k & 1);
+                      if (col >= st[h].col1 || (EXCL && col >= st[h].ex_lo && col < st[h].ex_hi)) a[ai(h, c, k)] = kInf;
+                      mn = fminf(mn, a[ai(h, c, k)]);
+                    }
+                    cm[h][c] = mn;
                   }
-                  cm[h][c] = mn;
                 }
-              }
+            }
             // the quad's minima of all eight chunks, one batch of independent whole-warp shuffles
 #pragma unroll
             for (int h = 0; h < 2; h++)
@@ -822,30 +829,26 @@ pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
               }
             }
             // events: the chunks inside the row's threshold after the tile (the one the drain applies), each with
-            // the exact mask of its columns inside it, so the re-rank touches only rows inside the window.  Built by
-            // the whole warp: shuffles inside the divergent event branch make ptxas serialise the wgmma.
-            uint32_t mk[2][kEvSlots];
+            // the exact mask of its columns inside it, so the re-rank touches only rows inside the window.  A row has
+            // about one event chunk in a tile with an event, so the mask of (row half h, chunk c) is built only when
+            // some row of the warp has an event there: the branch is warp-uniform, because shuffles inside a
+            // divergent branch make ptxas serialise the wgmma.
 #pragma unroll
             for (int h = 0; h < 2; h++)
 #pragma unroll
               for (int c = 0; c < kEvSlots; c++) {
-                mk[h][c] = 0;
+                const bool event = st[h].valid_row && cm[h][c] <= st[h].thr && cm[h][c] < kInf;
+                if (__any_sync(0xffffffffu, event)) {
+                  uint32_t mk = 0;
 #pragma unroll
-                for (int k = 0; k < 8; k++)
-                  mk[h][c] |= (a[ai(h, c, k)] <= st[h].thr) ? (1u << (8 * (k >> 1) + 2 * sub + (k & 1))) : 0u;
-              }
-#pragma unroll
-            for (int h = 0; h < 2; h++)
-#pragma unroll
-              for (int c = 0; c < kEvSlots; c++) mk[h][c] |= __shfl_xor_sync(0xffffffffu, mk[h][c], 1);
-#pragma unroll
-            for (int h = 0; h < 2; h++)
-#pragma unroll
-              for (int c = 0; c < kEvSlots; c++) {
-                mk[h][c] |= __shfl_xor_sync(0xffffffffu, mk[h][c], 2);
-                if (st[h].valid_row && cm[h][c] <= st[h].thr && cm[h][c] < kInf) {
-                  ev[h] |= 1 << c;
-                  if (sub == 0) eb->rec[(row_h0 + 8 * h) * kEvSlots + c] = EvRecord{col_base + 32 * c, mk[h][c], cm[h][c], st[h].thr};
+                  for (int k = 0; k < 8; k++)
+                    mk |= (a[ai(h, c, k)] <= st[h].thr) ? (1u << (8 * (k >> 1) + 2 * sub + (k & 1))) : 0u;
+                  mk |= __shfl_xor_sync(0xffffffffu, mk, 1);
+                  mk |= __shfl_xor_sync(0xffffffffu, mk, 2);
+                  if (event) {
+                    ev[h] |= 1 << c;
+                    if (sub == 0) eb->rec[(row_h0 + 8 * h) * kEvSlots + c] = EvRecord{col_base + 32 * c, mk, cm[h][c], st[h].thr};
+                  }
                 }
               }
           }
