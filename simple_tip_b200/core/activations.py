@@ -120,17 +120,9 @@ class HookedModelHandler:
     def _synced(self, fn, timer):
         """fn() timed by `timer`, which stops after a synchronise of the current CUDA device (the scoring device)
         and of the model's device when that is another CUDA device."""
-        import torch
-
         from .. import engine as E
 
-        score_dev, model_dev = E.require_cuda(), self._model_device()
-        with timer:
-            res = fn()
-            torch.cuda.synchronize(score_dev)
-            if model_dev.type == "cuda" and model_dev != score_dev:
-                torch.cuda.synchronize(model_dev)
-        return res
+        return _synced(fn, timer, E.require_cuda(), self._model_device())
 
 
 DROPOUT_SAMPLE_SIZE = 200      # handler_model.py:7
@@ -241,19 +233,34 @@ def _head_tensors(layers: Sequence[HeadLayer], dev):
     return out
 
 
-def head_input(trunk: Sequence, n: int):
+def head_input(trunk: Sequence, n: int, models: Optional[int] = None):
     """The head's input captured batch by batch in the point pass, as one [n, D] tensor; ValueError unless every
-    batch is 2-D float32 (a head of dense layers takes flat rows) and they hold n rows together."""
+    batch is 2-D float32 (a head of dense layers takes flat rows) and they hold n rows together.  With `models`, every
+    batch is a stack's [models, B, D] chunk and the result is [models, n, D]."""
     import torch
 
+    dims, want = (2, "2-D float32 [N, D]") if models is None else (3, f"3-D float32 [{models}, B, D]")
     for t in trunk:
-        if t.dim() != 2 or t.dtype != torch.float32:
-            raise ValueError(f"sampler='head' needs the head's input as 2-D float32 [N, D], got {tuple(t.shape)} "
-                             f"{t.dtype}")
-    h = torch.cat(list(trunk), dim=0) if len(trunk) != 1 else trunk[0]
-    if h.shape[0] != n:
-        raise ValueError(f"the head saw {h.shape[0]} rows, the model's output has {n}")
+        if t.dim() != dims or t.dtype != torch.float32 or (models is not None and t.shape[0] != models):
+            raise ValueError(f"sampler='head' needs the head's input as {want}, got {tuple(t.shape)} {t.dtype}")
+    rows = dims - 2
+    h = torch.cat(list(trunk), dim=rows) if len(trunk) != 1 else trunk[0]
+    if h.shape[rows] != n:
+        raise ValueError(f"the head saw {h.shape[rows]} rows, the model's output has {n}")
     return h
+
+
+def _synced(fn, timer, score_dev, model_dev):
+    """fn() timed by `timer`, which stops after a synchronise of the scoring device and of the model's device when
+    that is another CUDA device."""
+    import torch
+
+    with timer:
+        res = fn()
+        torch.cuda.synchronize(score_dev)
+        if model_dev.type == "cuda" and model_dev != score_dev:
+            torch.cuda.synchronize(model_dev)
+    return res
 
 
 def get_pred_and_uncertainty(model, x, batch_size: int = 32, sample_size: int = DROPOUT_SAMPLE_SIZE, seed: int = 0,
@@ -291,114 +298,7 @@ def get_pred_and_uncertainty(model, x, batch_size: int = 32, sample_size: int = 
     rows per launch, fed to the same vote kernels.  Its masks are this library's counter-based draws keyed by
     (seed, layer, row, sample, unit), not torch's, and dropouts nested in the trunk (the IMDB transformer block's)
     are not sampled, as in uncertainty-wizard; times["VR"] = [0, head-kernel time, vote time, 0]."""
-    import torch
-    from torch.nn.modules.dropout import _DropoutNd
-
-    from . import quantifiers as Q
-    from .deepgini import DeepGini
-    from .timer import Timer
-    from .. import engine as E
-
-    sampler = sampler if sampler is not None else os.environ.get("B200TIP_MC", "torch")
-    if sampler not in MC_SAMPLERS:
-        raise ValueError(f"sampler must be one of {MC_SAMPLERS}, got {sampler!r}")
-    head_at, head = mc_head_layers(model) if sampler == "head" else (-1, [])
-    score_dev = E.require_cuda()
-    dev = next(iter(model.parameters()), torch.empty(0)).device
-    if not isinstance(x, torch.Tensor):
-        x = torch.from_numpy(np.ascontiguousarray(x))
-    if x.shape[0] == 0:
-        raise ValueError("x holds no inputs")
-    x = x.to(dev)
-
-    def synced(fn, timer):
-        with timer:
-            res = fn()
-            torch.cuda.synchronize(score_dev)
-            if dev.type == "cuda" and dev != score_dev:
-                torch.cuda.synchronize(dev)
-        return res
-
-    modes = [(m, m.training) for m in model.modules()]
-    uncertainties: Dict[str, np.ndarray] = {}
-    times: Dict[str, List[float]] = {}
-    trunk: List[torch.Tensor] = []
-    hook = (list(model.children())[head_at].register_forward_pre_hook(lambda _m, inp: trunk.append(inp[0].detach()))
-            if head else None)
-    try:
-        pred_timer = Timer()
-        try:
-            probs = synced(lambda: TransparentModel(model, [], include_last_layer=True).collect(x, batch_size)[0],
-                           pred_timer)
-        finally:
-            if hook is not None:
-                hook.remove()
-        pred = None
-        for q in (Q.MaxSoftmax, Q.PredictionConfidenceScore, Q.SoftmaxEntropy, DeepGini):
-            timer = Timer()
-            q_pred, values = synced(lambda: q.calculate(probs), timer)
-            if pred is None:
-                pred = q_pred
-            name = q.aliases()[0].replace("custom::", "")
-            uncertainties[name] = q.cast_conf_or_unc(False, values)
-            times[name] = [0, pred_timer.get(), timer.get(), 0]
-
-        dropouts = [m for m in model.modules() if isinstance(m, _DropoutNd)]
-        if head:
-            h = E.to_device(head_input(trunk, probs.shape[0]), score_dev)
-            n, c = probs.shape
-            layers = _head_tensors(head, score_dev)
-            votes = Q.Votes(n, c, score_dev)
-            head_timer, vote_timer = Timer(), Timer()
-            for start in range(0, n if sample_size >= 1 else 0, MC_ROWS_PER_PASS):
-                b = min(MC_ROWS_PER_PASS, n - start)
-                out = synced(lambda: E.mc_head(h[start:start + b], layers, seed, sample_size, row0=start),
-                             head_timer)
-                if out.shape[2] != c:
-                    raise ValueError(f"the head gives {out.shape[2]} classes, the model's output {c}")
-                synced(lambda: votes.add(out, sample_size, sample_stride=c, row_stride=sample_size * c, row0=start,
-                                         rows=b), vote_timer)
-            _, vr = synced(lambda: votes.finish(sample_size), vote_timer)
-            uncertainties["VR"] = vr
-            times["VR"] = [0, head_timer.get(), vote_timer.get(), 0]
-        elif dropouts:
-            n, c = probs.shape
-            votes = Q.Votes(n, c, score_dev)
-            sampling_timer, vote_timer = Timer(), Timer()
-            model.eval()
-            for m in dropouts:
-                m.train()
-            with torch.random.fork_rng(devices=[dev] if dev.type == "cuda" else []), torch.no_grad():
-                torch.default_generator.manual_seed(seed)
-                if dev.type == "cuda":
-                    with torch.cuda.device(dev):
-                        torch.cuda.manual_seed(seed)
-                for start in range(0, n, batch_size):
-                    xb = x[start:start + batch_size]
-                    b = xb.shape[0]
-                    done = 0
-                    while done < sample_size:
-                        r = min(sample_size - done, max(1, MC_ROWS_PER_PASS // b))
-                        # row i * r + j of the pass is replica j of input i: [b, r, C] once viewed
-                        xr = xb.unsqueeze(1).expand(b, r, *xb.shape[1:]).reshape(b * r, *xb.shape[1:])
-                        out = synced(lambda: model(xr).detach(), sampling_timer)
-                        if tuple(out.shape) != (b * r, c):
-                            raise ValueError(f"an MC-dropout pass returned {tuple(out.shape)}, expected {(b * r, c)}")
-
-                        def vote():
-                            o = out if out.dtype in (torch.float32, torch.float64) else out.to(torch.float32)
-                            votes.add(E.to_device(o, score_dev), r, sample_stride=c, row_stride=r * c, row0=start,
-                                      rows=b)
-                        synced(vote, vote_timer)
-                        done += r
-            _, vr = synced(lambda: votes.finish(sample_size), vote_timer)
-            uncertainties["VR"] = vr
-            times["VR"] = [0, sampling_timer.get(), vote_timer.get(), 0]
-    finally:
-        for m, training in modes:
-            m.training = training
-    return pred, uncertainties, times
-
+    return _pred_and_uncertainty(model, x, batch_size, sample_size, [seed], sampler, stacked=False)[0]
 
 
 def get_pred_and_uncertainty_stack(stack, x, batch_size: int = 32, sample_size: int = DROPOUT_SAMPLE_SIZE,
@@ -424,13 +324,6 @@ def get_pred_and_uncertainty_stack(stack, x, batch_size: int = 32, sample_size: 
     quantifier time / M, 0] (for "VR": sampling and vote time / M).  Every module's mode is restored afterwards.
     ValueError, before any work, for a module that is not a StackedSequential, a seed count other than M, an
     unknown sampler, a head the head sampler cannot sample, or an empty x."""
-    import torch
-    from torch.nn.modules.dropout import _DropoutNd
-
-    from . import quantifiers as Q
-    from .deepgini import DeepGini
-    from .timer import Timer
-    from .. import engine as E
     from ..case_studies.stacked import StackedSequential
 
     if not isinstance(stack, StackedSequential):
@@ -439,59 +332,69 @@ def get_pred_and_uncertainty_stack(stack, x, batch_size: int = 32, sample_size: 
     seeds = [0] * n_models if seeds is None else [int(s) for s in seeds]
     if len(seeds) != n_models:
         raise ValueError(f"{len(seeds)} seeds for a stack of {n_models} models")
+    return _pred_and_uncertainty(stack, x, batch_size, sample_size, seeds, sampler, stacked=True)
+
+
+def _pred_and_uncertainty(model, x, batch_size: int, sample_size: int, seeds: List[int], sampler: Optional[str],
+                          stacked: bool) -> List[Tuple[np.ndarray, Dict[str, np.ndarray], Dict[str, List[float]]]]:
+    """What `get_pred_and_uncertainty` and `get_pred_and_uncertainty_stack` compute, for M = len(seeds) models in the
+    [M, N, C] layout: the M models of a StackedSequential when `stacked`, else one model (M = 1) whose outputs gain a
+    leading axis.  Returns one (pred, uncertainties, times) triple per model, each phase's time split evenly over
+    the M models."""
+    import torch
+    from torch.nn.modules.dropout import _DropoutNd
+
+    from . import quantifiers as Q
+    from .deepgini import DeepGini
+    from .timer import Timer
+    from .. import engine as E
+
     sampler = sampler if sampler is not None else os.environ.get("B200TIP_MC", "torch")
     if sampler not in MC_SAMPLERS:
         raise ValueError(f"sampler must be one of {MC_SAMPLERS}, got {sampler!r}")
-    head_at, head = mc_head_layers_stack(stack) if sampler == "head" else (-1, [])
+    head_at, head = (mc_head_layers_stack if stacked else mc_head_layers)(model) if sampler == "head" else (-1, [])
     score_dev = E.require_cuda()
-    dev = next(iter(stack.parameters()), torch.empty(0)).device
+    dev = next(iter(model.parameters()), torch.empty(0)).device
     if not isinstance(x, torch.Tensor):
         x = torch.from_numpy(np.ascontiguousarray(x))
     if x.shape[0] == 0:
         raise ValueError("x holds no inputs")
     x = x.to(dev)
-    n = x.shape[0]
-
-    def synced(fn, timer):
-        with timer:
-            res = fn()
-            torch.cuda.synchronize(score_dev)
-            if dev.type == "cuda" and dev != score_dev:
-                torch.cuda.synchronize(dev)
-        return res
+    n, n_models = x.shape[0], len(seeds)
 
     def forward(xb):
-        return stack(stack.stack_inputs([xb] * n_models)).detach()
+        """every model's output on the batch xb, [M, b, C]"""
+        if stacked:
+            return model(model.stack_inputs([xb] * n_models)).detach()
+        return model(xb).detach()[None]
 
     def point_pass():
-        outs = []
         with torch.no_grad():
-            for start in range(0, n, batch_size):
-                outs.append(forward(x[start:start + batch_size]))
+            outs = [forward(x[start:start + batch_size]) for start in range(0, n, batch_size)]
         return torch.cat(outs, dim=1) if len(outs) != 1 else outs[0]
 
-    modes = [(m, m.training) for m in stack.modules()]
+    modes = [(m, m.training) for m in model.modules()]
     uncertainties: List[Dict[str, np.ndarray]] = [{} for _ in range(n_models)]
     times: List[Dict[str, List[float]]] = [{} for _ in range(n_models)]
     trunk: List[torch.Tensor] = []
-    hook = (list(stack.children())[head_at].register_forward_pre_hook(lambda _m, inp: trunk.append(inp[0].detach()))
+    hook = (list(model.children())[head_at].register_forward_pre_hook(lambda _m, inp: trunk.append(inp[0].detach()))
             if head else None)
     try:
-        stack.eval()
+        model.eval()
         pred_timer = Timer()
         try:
-            probs = synced(point_pass, pred_timer)
+            probs = _synced(point_pass, pred_timer, score_dev, dev)
         finally:
             if hook is not None:
                 hook.remove()
         if probs.dim() != 3 or probs.shape[:2] != (n_models, n):
-            raise ValueError(f"the stack returned {tuple(probs.shape)}, expected [{n_models}, {n}, classes]")
+            raise ValueError(f"the model returned {tuple(probs.shape)}, expected [{n_models}, {n}, classes]")
         c = probs.shape[2]
         flat = probs.reshape(n_models * n, c)
         pred = None
         for q in (Q.MaxSoftmax, Q.PredictionConfidenceScore, Q.SoftmaxEntropy, DeepGini):
             timer = Timer()
-            q_pred, values = synced(lambda: q.calculate(flat), timer)
+            q_pred, values = _synced(lambda: q.calculate(flat), timer, score_dev, dev)
             if pred is None:
                 pred = q_pred.reshape(n_models, n)
             name = q.aliases()[0].replace("custom::", "")
@@ -500,57 +403,55 @@ def get_pred_and_uncertainty_stack(stack, x, batch_size: int = 32, sample_size: 
                 uncertainties[m][name] = values[m]
                 times[m][name] = [0, pred_timer.get() / n_models, timer.get() / n_models, 0]
 
-        dropouts = [m for m in stack.modules() if isinstance(m, _DropoutNd)]
-        votes = Q.Votes(n_models * n, c, score_dev) if head or dropouts else None
-        sampling_timer, vote_timer = Timer(), Timer()
-
-        def vote(out, samples, start, rows):
-            # out [M, rows, samples, C] (or its [M, rows * samples, C] view); model m's rows are votes rows m * n + i
-            for m in range(n_models):
-                votes.add(out[m], samples, sample_stride=c, row_stride=samples * c, row0=m * n + start, rows=rows)
-
-        if head:
-            for t in trunk:
-                if t.dim() != 3 or t.dtype != torch.float32 or t.shape[0] != n_models:
-                    raise ValueError(f"sampler='head' needs the head's input as 3-D float32 [{n_models}, B, D], got "
-                                     f"{tuple(t.shape)} {t.dtype}")
-            h = E.to_device(torch.cat(trunk, dim=1) if len(trunk) != 1 else trunk[0], score_dev)
-            if h.shape[1] != n:
-                raise ValueError(f"the head saw {h.shape[1]} rows, the stack's output has {n}")
-            layers = _head_tensors(head, score_dev)
-            rows_per_pass = max(1, MC_ROWS_PER_PASS // n_models)
-            for start in range(0, n if sample_size >= 1 else 0, rows_per_pass):
-                b = min(rows_per_pass, n - start)
-                out = synced(lambda: E.mc_head_stack(h[:, start:start + b], layers, seeds, sample_size, row0=start),
-                             sampling_timer)
-                if out.shape[3] != c:
-                    raise ValueError(f"the head gives {out.shape[3]} classes, the stack's output {c}")
-                synced(lambda: vote(out, sample_size, start, b), vote_timer)
-        elif dropouts:
-            for m in dropouts:
-                m.train()
-            with torch.random.fork_rng(devices=[dev] if dev.type == "cuda" else []), torch.no_grad():
-                torch.default_generator.manual_seed(seeds[0])
-                if dev.type == "cuda":
-                    with torch.cuda.device(dev):
-                        torch.cuda.manual_seed(seeds[0])
-                for start in range(0, n, batch_size):
-                    xb = x[start:start + batch_size]
-                    b = xb.shape[0]
-                    done = 0
-                    while done < sample_size:
-                        r = min(sample_size - done, max(1, MC_ROWS_PER_PASS // (b * n_models)))
-                        # row i * r + j of a model's pass is replica j of input i: [b, r, C] once viewed
-                        xr = xb.unsqueeze(1).expand(b, r, *xb.shape[1:]).reshape(b * r, *xb.shape[1:])
-                        out = synced(lambda: forward(xr), sampling_timer)
-                        if tuple(out.shape) != (n_models, b * r, c):
-                            raise ValueError(f"an MC-dropout pass returned {tuple(out.shape)}, expected "
-                                             f"{(n_models, b * r, c)}")
-                        o = out if out.dtype in (torch.float32, torch.float64) else out.to(torch.float32)
-                        synced(lambda: vote(E.to_device(o, score_dev), r, start, b), vote_timer)
-                        done += r
+        dropouts = [m for m in model.modules() if isinstance(m, _DropoutNd)]
         if head or dropouts:
-            _, vr = synced(lambda: votes.finish(sample_size), vote_timer)
+            votes = Q.Votes(n_models * n, c, score_dev)
+            sampling_timer, vote_timer = Timer(), Timer()
+
+            def vote(out, samples, start, rows):
+                # out [M, rows, samples, C] (or its [M, rows * samples, C] view); model m's rows are votes rows m * n + i
+                for m in range(n_models):
+                    votes.add(out[m], samples, sample_stride=c, row_stride=samples * c, row0=m * n + start, rows=rows)
+
+            if head:
+                h = E.to_device(head_input(trunk, n, n_models) if stacked else head_input(trunk, n)[None], score_dev)
+                layers = _head_tensors(head, score_dev)
+                rows_per_pass = max(1, MC_ROWS_PER_PASS // n_models)
+                for start in range(0, n if sample_size >= 1 else 0, rows_per_pass):
+                    b = min(rows_per_pass, n - start)
+
+                    def sample():
+                        if stacked:
+                            return E.mc_head_stack(h[:, start:start + b], layers, seeds, sample_size, row0=start)
+                        return E.mc_head(h[0, start:start + b], layers, seeds[0], sample_size, row0=start)[None]
+                    out = _synced(sample, sampling_timer, score_dev, dev)
+                    if out.shape[3] != c:
+                        raise ValueError(f"the head gives {out.shape[3]} classes, the model's output {c}")
+                    _synced(lambda: vote(out, sample_size, start, b), vote_timer, score_dev, dev)
+            else:
+                for m in dropouts:
+                    m.train()
+                with torch.random.fork_rng(devices=[dev] if dev.type == "cuda" else []), torch.no_grad():
+                    torch.default_generator.manual_seed(seeds[0])
+                    if dev.type == "cuda":
+                        with torch.cuda.device(dev):
+                            torch.cuda.manual_seed(seeds[0])
+                    for start in range(0, n, batch_size):
+                        xb = x[start:start + batch_size]
+                        b = xb.shape[0]
+                        done = 0
+                        while done < sample_size:
+                            r = min(sample_size - done, max(1, MC_ROWS_PER_PASS // (b * n_models)))
+                            # row i * r + j of a model's pass is replica j of input i: [b, r, C] once viewed
+                            xr = xb.unsqueeze(1).expand(b, r, *xb.shape[1:]).reshape(b * r, *xb.shape[1:])
+                            out = _synced(lambda: forward(xr), sampling_timer, score_dev, dev)
+                            if tuple(out.shape) != (n_models, b * r, c):
+                                raise ValueError(f"an MC-dropout pass returned {tuple(out.shape)}, expected "
+                                                 f"{(n_models, b * r, c)}")
+                            o = out if out.dtype in (torch.float32, torch.float64) else out.to(torch.float32)
+                            _synced(lambda: vote(E.to_device(o, score_dev), r, start, b), vote_timer, score_dev, dev)
+                            done += r
+            _, vr = _synced(lambda: votes.finish(sample_size), vote_timer, score_dev, dev)
             vr = vr.reshape(n_models, n)
             for m in range(n_models):
                 uncertainties[m]["VR"] = vr[m]

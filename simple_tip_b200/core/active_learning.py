@@ -281,23 +281,7 @@ def accuracy(model, x, y, batch_size: int = 128) -> float:
     """What Keras' `model.evaluate(x, y)[1]` is for the study's softmax models: the share of inputs whose first-index
     argmax of the output equals the label, as the exact `correct / n`.  The model runs where its parameters live,
     in eval mode without gradients, in batches of `batch_size`; its modes are restored afterwards."""
-    import torch
-
-    dev = next(iter(model.parameters()), torch.empty(0)).device
-    labels = _as_tensor(y, dev).reshape(-1)
-    n = labels.shape[0]
-    modes = [(m, m.training) for m in model.modules()]
-    correct = torch.zeros((), dtype=torch.int64, device=dev)
-    model.eval()
-    try:
-        with torch.no_grad():
-            for start in range(0, n, batch_size):
-                out = model(_as_tensor(x[start:start + batch_size], dev))
-                correct += (out.argmax(dim=1) == labels[start:start + batch_size]).sum()
-    finally:
-        for m, training in modes:
-            m.training = training
-    return int(correct.item()) / n
+    return _accuracies(model, 1, lambda xb: model(xb)[None], x, y, batch_size)[0]
 
 
 def accuracies_stack(stack, x, y, batch_size: int = 128) -> list:
@@ -305,25 +289,38 @@ def accuracies_stack(stack, x, y, batch_size: int = 128) -> list:
     from one stacked forward per batch of `batch_size`: model m's exact correct / n, its correct count summed from the
     first-index argmax of its slice [b, classes] of the stacked softmax output.  The stack runs in eval mode without
     gradients; its modes are restored afterwards."""
+    m = len(stack.sources)
+    return _accuracies(stack, m, lambda xb: stack(stack.stack_inputs([xb] * m)), x, y, batch_size)
+
+
+def _accuracies(model, models: int, forward, x, y, batch_size: int) -> list:
+    """Each model's exact correct / n, where forward(batch) gives the M = `models` outputs [M, b, classes] of
+    `model`, which runs in eval mode without gradients and has its modes restored afterwards."""
     import torch
 
-    m = len(stack.sources)
-    dev = next(iter(stack.parameters()), torch.empty(0)).device
+    dev = next(iter(model.parameters()), torch.empty(0)).device
     labels = _as_tensor(y, dev).reshape(-1)
     n = labels.shape[0]
-    modes = [(module, module.training) for module in stack.modules()]
-    correct = torch.zeros(m, dtype=torch.int64, device=dev)
-    stack.eval()
+    modes = [(module, module.training) for module in model.modules()]
+    correct = torch.zeros(models, dtype=torch.int64, device=dev)
+    model.eval()
     try:
         with torch.no_grad():
             for start in range(0, n, batch_size):
-                xb = _as_tensor(x[start:start + batch_size], dev)
-                out = stack(stack.stack_inputs([xb] * m))                # [M, b, classes]
+                out = forward(_as_tensor(x[start:start + batch_size], dev))
                 correct += (out.argmax(dim=2) == labels[start:start + batch_size]).sum(dim=1)
     finally:
         for module, training in modes:
             module.training = training
     return [int(c) / n for c in correct.tolist()]
+
+
+def _checked(acc: float) -> float:
+    assert 0 <= acc <= 1, (
+        "The models metric is not accuracy, change your "
+        "training_process callable."
+    )
+    return acc
 
 
 def _evaluate_stack(models: Sequence, datasets: SplitDataset, num_classes: Optional[int], batch_size: int = 128
@@ -338,24 +335,12 @@ def _evaluate_stack(models: Sequence, datasets: SplitDataset, num_classes: Optio
         return [_evaluate(m, datasets, num_classes, batch_size) for m in models]
     net = stack(models)
     res = [dict() for _ in models]
-    for (ood_or_nom, observed_or_future), (x, y) in datasets.items():
+    for key, (x, y) in datasets.items():
         for eval_res, acc in zip(res, accuracies_stack(net, x, y, batch_size)):
-            assert 0 <= acc <= 1, (
-                "The models metric is not accuracy, change your "
-                "training_process callable."
-            )
-            eval_res[ood_or_nom, observed_or_future] = acc
+            eval_res[key] = _checked(acc)
     return res
 
 
 def _evaluate(model, datasets: SplitDataset, num_classes: Optional[int], batch_size: int = 128) -> SplitEvaluation:
     """eval_active_learning.py:299-313: the model's accuracy on all four splits."""
-    res: SplitEvaluation = dict()
-    for (ood_or_nom, observed_or_future), (x, y) in datasets.items():
-        acc = accuracy(model, x, y, batch_size)
-        assert 0 <= acc <= 1, (
-            "The models metric is not accuracy, change your "
-            "training_process callable."
-        )
-        res[ood_or_nom, observed_or_future] = acc
-    return res
+    return {key: _checked(accuracy(model, x, y, batch_size)) for key, (x, y) in datasets.items()}

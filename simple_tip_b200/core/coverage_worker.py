@@ -8,14 +8,16 @@ device and nothing is written to disk.
 """
 from __future__ import annotations
 
+import functools
+import math
 from typing import Dict, List, Sequence, Tuple
 
 import numpy as np
 
+from . import prioritizers as P
 from .activations import HookedModelHandler, TransparentModel
 from .aggregate_statistics import AggregateStatisticsCollector
 from .neuron_coverage import KMNC, NAC, NBC, SNAC, TKNC, CoverageMethod, _score_dtype
-from .prioritizers import cam_from_bits, cam_from_bits_stack
 from .timer import Timer
 
 # The study's twelve coverage metrics (handler_coverage.py:49-101) as (id, debit, factory): the factory builds the
@@ -37,7 +39,139 @@ def _walk_debits(agg_stats: AggregateStatisticsCollector, pred_timer: Timer) -> 
     return {"NBC": mn + mx + pred + wf, "SNAC": wf + mx + pred, "KMNC": mn + mx + pred, None: 0.0}
 
 
-class CoverageWorker(HookedModelHandler):
+class _CoverageArm(HookedModelHandler):
+    """What `CoverageWorker` and `StackedCoverageWorker` share: the coverage arm of the M models hooked in
+    `self.base_model`, all fed the same inputs.  A subclass sets `models`, `base_model` and `batch_size` and gives
+    `_activations(badge)`, every hooked layer of one forward on the badge as [M, b, *layer shape], and
+    `_cam(scores, bits)`, the M CAM orders of M profiles."""
+
+    models = 1
+
+    def _walk(self, training_data):
+        """The training walk (handler_coverage.py:33-42) and the metrics of `METRICS`.  Every hooked output goes to one
+        `AggregateStatisticsCollector` as rows [b, M, *layer shape], so one `tip_stats_update` per layer and badge
+        serves all M models.  Sets `self._metrics` (per metric, one object per model, or one for all M models when
+        the metric holds no state) and `self.setup_times` (split evenly over the M models); returns (mins, maxs,
+        stds), each per model a list of layer-shaped arrays."""
+        x = self._inputs(training_data, "training_data")
+        agg_stats = AggregateStatisticsCollector()
+        pred_timer = Timer()
+        for start in range(0, x.shape[0], self.batch_size):
+            activations = self._synced(lambda: self._activations(x[start:start + self.batch_size]), pred_timer)
+            agg_stats.track([a.transpose(0, 1) for a in activations])     # [b, M, *layer shape]
+        mins, maxs, stds = ([[layer[m] for layer in stat] for m in range(self.models)] for stat in agg_stats.get())
+
+        debits = _walk_debits(agg_stats, pred_timer)
+        self._metrics: Dict[str, List[CoverageMethod]] = {}
+        self.setup_times: Dict[str, float] = {}
+        for metric_id, debit, factory in METRICS:
+            timer = Timer()
+            built = range(1 if debit is None else self.models)
+            self._metrics[metric_id] = self._synced(lambda: [factory(mins[m], maxs[m], stds[m]) for m in built], timer)
+            self.setup_times[metric_id] = (debits[debit] + timer.get()) / self.models
+        return mins, maxs, stds
+
+    def _traces(self, data):
+        """The test set's traces as one model-major [M, N, D] tensor on the scoring device (each model's layers
+        flattened and concatenated in layer order, in the dtype `torch.cat` of the layers gives), and each layer's
+        shape."""
+        import torch
+
+        from .. import engine as E
+
+        dev = E.require_cuda()
+        x = self._inputs(data, "test data")
+        n = int(x.shape[0])
+        flat, shapes = None, None
+        for start in range(0, n, self.batch_size):
+            acts = self._activations(x[start:start + self.batch_size])
+            if flat is None:
+                shapes = [tuple(a.shape[2:]) for a in acts]
+                dtype = functools.reduce(torch.promote_types, [a.dtype for a in acts])
+                flat = torch.empty((self.models, n, sum(math.prod(s) for s in shapes)), dtype=dtype, device=dev)
+            off = 0
+            for a in acts:
+                a = a.reshape(a.shape[0], a.shape[1], -1)
+                flat[:, start:start + a.shape[1], off:off + a.shape[2]].copy_(a)
+                off += a.shape[2]
+        return flat, shapes
+
+    def _model_major(self, data):
+        """What `_evaluate` scores: `_traces`' [M, N, D] tensor and layer shapes."""
+        return self._traces(data)
+
+    @staticmethod
+    def _cam_sanity_check(cam_order, scores):
+        assert len(cam_order) == len(set(cam_order)) == scores.shape[0], "CAM order is not unique or not complete"
+
+    def _evaluate(self, test_dataset
+                  ) -> List[Tuple[Dict[str, List[float]], Dict[str, np.ndarray], Dict[str, np.ndarray]]]:
+        """M (times, all_scores, cam_orders) triples in `CoverageWorker.evaluate_all`'s form, each phase's time split
+        evenly over the M models.  NAC runs once on the traces' [M * N, D] view, NBC, SNAC and KMNC on each model's
+        [N, D] slice, TKNC on each model's layer views."""
+        import torch
+
+        from .. import _lib
+
+        models = self.models
+        pred_timer = Timer()
+        flat, shapes = self._synced(lambda: self._model_major(test_dataset), pred_timer)
+        n, d = int(flat.shape[1]), int(flat.shape[2])
+        widths = [math.prod(s) for s in shapes]
+        words = int(_lib.load().tip_cover_packed_words(d))
+        results = [({}, {}, {}) for _ in range(models)]
+        copies = {}
+
+        def layers(m):
+            """model m's layers as contiguous [N, w] copies (`tip_tknc` reads contiguous rows), kept for the next TKNC
+            metric; one model's copies at a time"""
+            if m not in copies:
+                copies.clear()
+                copies[m] = [t.contiguous() for t in flat[m].split(widths, dim=1)]
+            return copies[m]
+
+        for metric_id, metric in self._metrics.items():
+            if not isinstance(metric[0], TKNC):
+                copies.clear()
+            quant_timer = Timer()
+
+            def quant():
+                if isinstance(metric[0], NAC):                  # one launch over the [M * N, D] view
+                    score, bits = metric[0].packed(flat.view(models * n, d))
+                    score, bits = score.view(models, n), bits.view(models, n, -1)
+                else:
+                    score, bits = None, None
+                    for m in range(models):
+                        if isinstance(metric[0], TKNC):
+                            s, b = metric[0].packed(layers(m))
+                        else:
+                            s, b = metric[m].packed(flat[m])
+                        if models == 1:                         # one model's profile is taken as it is
+                            score, bits = s[None], b[None]
+                            continue
+                        if bits is None:
+                            score = torch.empty((models, n), dtype=s.dtype, device=s.device)
+                            bits = torch.empty((models, n, int(b.shape[1])), dtype=b.dtype, device=b.device)
+                        score[m].copy_(s)
+                        bits[m].copy_(b)
+                        del s, b
+                # sum_score's dtype: from the dense profile's entries per sample, d x planes
+                return score.cpu().numpy().astype(_score_dtype(d * (int(bits.shape[2]) // words))), bits
+            scores, bits = self._synced(quant, quant_timer)
+            cam_timer = Timer()
+            orders = self._synced(lambda: self._cam(scores, bits), cam_timer)
+            del bits
+            for m, order in enumerate(orders):
+                self._cam_sanity_check(order, scores[m])
+                times, all_scores, cam_orders = results[m]
+                times[metric_id] = [self.setup_times[metric_id], pred_timer.get() / models, quant_timer.get() / models,
+                                    cam_timer.get() / models]
+                all_scores[metric_id] = scores[m]
+                cam_orders[metric_id] = order
+        return results
+
+
+class CoverageWorker(_CoverageArm):
     """`CoverageWorker(base_model, training_set)` + `evaluate_all(test_dataset, test_dataset_id)` of
     handler_coverage.py for a `torch.nn.Module`.
 
@@ -61,40 +195,31 @@ class CoverageWorker(HookedModelHandler):
         self.nc_layers = list(nc_layers)
         self.base_model = TransparentModel(model, self.nc_layers, include_last_layer=False)
         self.batch_size = batch_size
-        self.metrics: Dict[str, CoverageMethod] = {}
-        self.setup_times: Dict[str, float] = {}
+        (self.mins,), (self.maxs,), (self.stds,) = self._walk(training_data)     # per layer, layer-shaped
+        self.metrics: Dict[str, CoverageMethod] = {metric_id: m[0] for metric_id, m in self._metrics.items()}
 
-        x = self._inputs(training_data, "training_data")
-        agg_stats = AggregateStatisticsCollector()
-        pred_timer = Timer()
-        for start in range(0, x.shape[0], batch_size):           # handler_coverage.py:33-42
-            badge = x[start:start + batch_size]
-            activations = self._synced(lambda: self.base_model.get_activations(badge), pred_timer)
-            agg_stats.track(activations)
-        mins, maxs, std = agg_stats.get()
-        self.mins, self.maxs, self.stds = mins, maxs, std          # per layer, layer-shaped
+    def _activations(self, badge):
+        return [a[None] for a in self.base_model.get_activations(badge)]
 
-        debits = _walk_debits(agg_stats, pred_timer)
-        for metric_id, debit, factory in METRICS:
-            timer = Timer()
-            self.metrics[metric_id] = self._synced(lambda: factory(mins, maxs, std), timer)
-            self.setup_times[metric_id] = debits[debit] + timer.get()
-
-    def _traces(self, data) -> Tuple[List, object]:
-        """The test set's hooked layers on the scoring device (moved there once if the model lives elsewhere), and
-        the same traces flattened to one [N, D] matrix, in input order."""
-        import torch
-
-        from .. import engine as E
-
-        dev = E.require_cuda()
-        layers = [a.to(dev) for a in self.base_model.collect(self._inputs(data, "test data"), self.batch_size)]
-        flat = torch.cat([a.reshape(a.shape[0], -1) for a in layers], dim=1)
+    def _traces(self, data):
+        """The test set's hooked layers on the scoring device, and the same traces flattened to one [N, D] matrix, in
+        input order; the layers are views of the matrix."""
+        flat, shapes = super()._traces(data)
+        flat = flat[0]
+        layers, off = [], 0
+        for shape in shapes:
+            width = math.prod(shape)
+            layers.append(flat[:, off:off + width].view(flat.shape[0], *shape))
+            off += width
         return layers, flat
 
+    def _model_major(self, data):
+        layers, flat = self._traces(data)
+        return flat[None], [tuple(a.shape[1:]) for a in layers]
+
     @staticmethod
-    def _cam_sanity_check(cam_order, scores):
-        assert len(cam_order) == len(set(cam_order)) == scores.shape[0], "CAM order is not unique or not complete"
+    def _cam(scores, bits):
+        return [np.array(list(P.cam_from_bits(scores[0], bits[0])), dtype=np.int64)]
 
     def evaluate_all(self, test_dataset, test_dataset_id=None
                      ) -> Tuple[Dict[str, List[float]], Dict[str, np.ndarray], Dict[str, np.ndarray]]:
@@ -106,29 +231,7 @@ class CoverageWorker(HookedModelHandler):
         cam = `cam_from_bits` on the packed profile.  all_scores[m]: NumPy, in the dtype the reference's `sum_score`
         picks; cam_orders[m]: int64.  Rows are in input order.  test_dataset_id is accepted for the reference's
         signature; nothing is written anywhere.  An empty test set raises ValueError before any launch."""
-        from .. import _lib
-
-        pred_timer = Timer()
-        layers, flat = self._synced(lambda: self._traces(test_dataset), pred_timer)
-        d = int(flat.shape[1])
-        words = int(_lib.load().tip_cover_packed_words(d))
-        times, all_scores, cam_orders = {}, {}, {}
-        for metric_id, metric in self.metrics.items():
-            quant_timer = Timer()
-
-            def quant():
-                score, bits = metric.packed(layers if isinstance(metric, TKNC) else flat)
-                # sum_score's dtype: from the dense profile's entries per sample, d x planes
-                return score.cpu().numpy().astype(_score_dtype(d * (int(bits.shape[1]) // words))), bits
-            scores, bits = self._synced(quant, quant_timer)
-            cam_timer = Timer()
-            order = self._synced(lambda: np.array(list(cam_from_bits(scores, bits)), dtype=np.int64), cam_timer)
-            self._cam_sanity_check(order, scores)
-            del bits
-            times[metric_id] = [self.setup_times[metric_id], pred_timer.get(), quant_timer.get(), cam_timer.get()]
-            all_scores[metric_id] = scores
-            cam_orders[metric_id] = order
-        return times, all_scores, cam_orders
+        return self._evaluate(test_dataset)[0]
 
 
 def stack_layer_ids(nc_layers: Sequence) -> List[int]:
@@ -141,7 +244,7 @@ def stack_layer_ids(nc_layers: Sequence) -> List[int]:
     return [int(lid) for lid in ids]
 
 
-class StackedCoverageWorker(HookedModelHandler):
+class StackedCoverageWorker(_CoverageArm):
     """`CoverageWorker` for the M models of a `case_studies.stacked.StackedSequential`, all on the same inputs.
 
     nc_layers: child indices of the stack (dotted submodule names raise ValueError before any forward pass).
@@ -175,104 +278,21 @@ class StackedCoverageWorker(HookedModelHandler):
         self.models = len(stack.sources)
         self.base_model = TransparentModel(stack, self.nc_layers, include_last_layer=False)
         self.batch_size = batch_size
-        self.metrics: Dict[str, List[CoverageMethod]] = {}
-        self.setup_times: Dict[str, float] = {}
-
-        x = self._inputs(training_data, "training_data")
-        agg_stats = AggregateStatisticsCollector()
-        pred_timer = Timer()
-        for start in range(0, x.shape[0], batch_size):
-            activations = self._synced(lambda: self._activations(x[start:start + batch_size]), pred_timer)
-            agg_stats.track([a.transpose(0, 1) for a in activations])     # [b, M, *layer shape]
-        mins, maxs, std = agg_stats.get()
-        m_range = range(self.models)
-        self.mins, self.maxs, self.stds = ([[layer[m] for layer in stat] for m in m_range] for stat in (mins, maxs, std))
-
-        debits = _walk_debits(agg_stats, pred_timer)
-        for metric_id, debit, factory in METRICS:
-            timer = Timer()
-            built = range(1) if debit is None else m_range        # a stateless metric: one object for all M models
-            self.metrics[metric_id] = self._synced(
-                lambda: [factory(self.mins[m], self.maxs[m], self.stds[m]) for m in built], timer)
-            self.setup_times[metric_id] = (debits[debit] + timer.get()) / self.models
+        self.mins, self.maxs, self.stds = self._walk(training_data)
+        self.metrics: Dict[str, List[CoverageMethod]] = self._metrics
 
     def _activations(self, badge):
         """The hooked layers of one stacked forward on `badge` (every model sees it), each [M, b, *layer shape]."""
         acts = self.base_model.get_activations(self.stack.stack_inputs([badge] * self.models))
         return [self.stack.model_major(child, a) for child, a in zip(self.nc_layers, acts)]
 
-    def _traces(self, data):
-        """The test set's traces as one model-major [M, N, D] tensor on the scoring device (each model's layers
-        flattened and concatenated in layer order, as `CoverageWorker` flattens them), and the layer widths."""
-        import torch
-
-        from .. import engine as E
-
-        dev = E.require_cuda()
-        x = self._inputs(data, "test data")
-        n = int(x.shape[0])
-        flat, widths = None, None
-        for start in range(0, n, self.batch_size):
-            acts = [a.reshape(a.shape[0], a.shape[1], -1) for a in self._activations(x[start:start + self.batch_size])]
-            if flat is None:
-                widths = [int(a.shape[2]) for a in acts]
-                flat = torch.empty((self.models, n, sum(widths)), dtype=acts[0].dtype, device=dev)
-            off = 0
-            for a, w in zip(acts, widths):
-                flat[:, start:start + a.shape[1], off:off + w].copy_(a)
-                off += w
-        return flat, widths
+    @staticmethod
+    def _cam(scores, bits):
+        return P.cam_from_bits_stack(list(scores), bits)
 
     def evaluate_all(self, test_dataset, test_dataset_id=None
                      ) -> List[Tuple[Dict[str, List[float]], Dict[str, np.ndarray], Dict[str, np.ndarray]]]:
         """M (times, all_scores, cam_orders) triples, model m's in `CoverageWorker.evaluate_all`'s form; times[metric]
         = [setup, pred, quant, cam] with each phase's stack time split evenly over the M models.  An empty test set
         raises ValueError before any launch."""
-        import torch
-
-        from .. import _lib
-
-        models = self.models
-        pred_timer = Timer()
-        flat, widths = self._synced(lambda: self._traces(test_dataset), pred_timer)
-        n, d = int(flat.shape[1]), int(flat.shape[2])
-        words = int(_lib.load().tip_cover_packed_words(d))
-        results = [({}, {}, {}) for _ in range(models)]
-        for metric_id, metric in self.metrics.items():
-            quant_timer = Timer()
-
-            def quant():
-                if isinstance(metric[0], NAC):                  # one launch over the [M * N, D] view
-                    score, bits = metric[0].packed(flat.view(models * n, d))
-                    score, bits = score.view(models, n), bits.view(models, n, -1)
-                else:
-                    score, bits = None, None
-                    for m in range(models):
-                        if isinstance(metric[0], TKNC):
-                            layers, off = [], 0
-                            for w in widths:
-                                layers.append(flat[m, :, off:off + w])
-                                off += w
-                            s, b = metric[0].packed(layers)
-                        else:
-                            s, b = metric[m].packed(flat[m])
-                        if bits is None:
-                            score = torch.empty((models, n), dtype=s.dtype, device=s.device)
-                            bits = torch.empty((models, n, int(b.shape[1])), dtype=b.dtype, device=b.device)
-                        score[m].copy_(s)
-                        bits[m].copy_(b)
-                        del s, b
-                # sum_score's dtype: from the dense profile's entries per sample, d x planes
-                return score.cpu().numpy().astype(_score_dtype(d * (int(bits.shape[2]) // words))), bits
-            scores, bits = self._synced(quant, quant_timer)
-            cam_timer = Timer()
-            orders = self._synced(lambda: cam_from_bits_stack(list(scores), bits), cam_timer)
-            del bits
-            for m, order in enumerate(orders):
-                CoverageWorker._cam_sanity_check(order, scores[m])
-                times, all_scores, cam_orders = results[m]
-                times[metric_id] = [self.setup_times[metric_id], pred_timer.get() / models, quant_timer.get() / models,
-                                    cam_timer.get() / models]
-                all_scores[metric_id] = scores[m]
-                cam_orders[metric_id] = order
-        return results
+        return self._evaluate(test_dataset)

@@ -289,3 +289,34 @@ def test_coverage_arm_result_files(worker_run, tmp_path):
             assert apfd[name][0] == apfd_from_order(m, np.argsort(-want_s))
             assert apfd[name + "-cam"][0] == apfd_from_order(m, np_oracle.cam_oracle(want_s, want_p))
             assert R.load_times(out, "toy", ds, 0, name) == times[name]
+
+
+def test_single_model_paths_never_run_the_stack_kernels(monkeypatch):
+    """One model's head sampler runs `engine.mc_head` and its coverage arm `prioritizers.cam_from_bits`, never their
+    stacked forms with M = 1."""
+    torch = _torch()
+    from simple_tip_b200 import engine as E
+    from simple_tip_b200.case_studies import mnist
+    from simple_tip_b200.core import prioritizers as P
+    from simple_tip_b200.core.activations import get_pred_and_uncertainty
+    from simple_tip_b200.core.coverage_worker import CoverageWorker
+
+    calls = []
+
+    def spy(name, fn):
+        def wrapped(*args, **kwargs):
+            calls.append(name)
+            return fn(*args, **kwargs)
+        monkeypatch.setattr(E if name.startswith("mc_") else P, name, wrapped)
+    for name in ("mc_head", "mc_head_stack"):
+        spy(name, getattr(E, name))
+    for name in ("cam_from_bits", "cam_from_bits_stack"):
+        spy(name, getattr(P, name))
+    torch.manual_seed(0)
+    model = mnist.network().cuda()
+    x = torch.rand(300, 28, 28, 1, device="cuda")
+    get_pred_and_uncertainty(model, x, batch_size=128, sample_size=8, sampler="head")
+    assert calls == ["mc_head"]
+    calls.clear()
+    CoverageWorker(model, mnist.NC_ACTIVATION_LAYERS, x, batch_size=BATCH).evaluate_all(x[:200])
+    assert calls == ["cam_from_bits"] * len(NAMES)
