@@ -17,13 +17,10 @@ online log-sum-exp) and converted back to a float64 density here, so underflow t
 from __future__ import annotations
 
 import math
-import os
 import warnings
 from typing import Optional
 
 import numpy as np
-
-GRAPHS = os.environ.get("B200TIP_GRAPHS", "1") != "0"   # CUDA-graph replay of repeated batch shapes
 
 
 class StableGaussianKDE:
@@ -162,6 +159,9 @@ class StableGaussianKDE:
         self._w_dev = w32.to(dev)
         self._mu_dev = mu.to(dev)
         self._cols_dev = None if self.source_columns is None else torch.from_numpy(self.source_columns).to(dev)
+        self._plans = E.BoundedCache(4)
+        self._seen_shapes = E.BoundedCache(65)
+        self._pinned_pool = E.BoundedCache(33)
 
     # -- score -----------------------------------------------------------------------------
     def evaluate(self, points) -> np.ndarray:
@@ -228,22 +228,15 @@ class StableGaussianKDE:
         # ten such chains per scoring call, handler_surprise.py:26).
         dt = (torch.float64 if rows.dtype in (torch.float64, np.float64) else torch.float32)
         key = (int(m), int(rows.shape[1]), dt, bool(preselected), fast)
-        plans = self.__dict__.setdefault("_plans", {})
-        seen = self.__dict__.setdefault("_seen_shapes", set())
-        plan = plans.get(key)
-        if plan is None and GRAPHS and eng.comm is None and key in seen:
-            if len(plans) >= 4:
-                plans.pop(next(iter(plans)))
-            plan = plans[key] = _DensityPlan(self, key)
+        plan = self._plans.get(key)
+        if plan is None and self._seen_shapes.touch(key) and E.GRAPHS and eng.comm is None:
+            plan = self._plans.get_or_make(key, lambda: _DensityPlan(self, key))
         if plan is not None:
             src = rows if isinstance(rows, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(rows))
             plan.x_in.copy_(src, non_blocking=True)
             plan.graph.replay()
             packed, n_s, q = plan.packed, plan.n_s, plan.q
         else:
-            if len(seen) > 64:
-                seen.clear()
-            seen.add(key)
             packed, n_s, q = self._density_body(E.to_device(rows, eng.dev), preselected, fast)
         host = self._pinned(packed.shape)
         host.copy_(packed, non_blocking=True)
@@ -259,6 +252,7 @@ class StableGaussianKDE:
 
         eng = self._engine
         m = x.shape[0]
+        E.keep_for_capture(self._cols_dev, self._mu_dev, self._w_dev)
         q = E.whiten(x, None if preselected else self._cols_dev, self._mu_dev, self._w_dev)
         if fast:
             eng.flags.zero_()
@@ -279,14 +273,7 @@ class StableGaussianKDE:
         import torch
 
         key = tuple(shape)
-        pool = self.__dict__.setdefault("_pinned_pool", {})
-        buf = pool.get(key)
-        if buf is None:
-            if len(pool) > 32:
-                pool.clear()
-            buf = torch.empty(key, dtype=torch.float64, pin_memory=True)
-            pool[key] = buf
-        return buf
+        return self._pinned_pool.get_or_make(key, lambda: torch.empty(key, dtype=torch.float64, pin_memory=True))
 
     def _finish(self, log_max: np.ndarray, rel_sum: np.ndarray) -> np.ndarray:
         """float64 density from the log-domain partials, with the reference's underflow:
@@ -306,37 +293,18 @@ class _DensityPlan:
     """One density evaluation of a fixed batch shape as a CUDA graph (see StableGaussianKDE._density_begin)."""
 
     def __init__(self, kde, key):
-        import gc
-
         import torch
 
+        from .. import engine as E
+
         m, d_in, dt, preselected, fast = key
-        eng = kde._engine
-        dev = eng.dev
+        dev = kde._engine.dev
         self.x_in = torch.zeros((m, d_in), dtype=dt, device=dev)
-        # engine-owned tensors whose addresses the graph bakes in (work lists are cached per batch size and may be
-        # evicted from the engine's cache later)
-        self.refs = [eng._work_items(m), kde._cols_dev, kde._mu_dev, kde._w_dev, eng.t_pack, eng.t_pack_f16, eng.flags]
-        if fast:
-            self.refs.append(eng._work_items(min(m, kde.FAST_SAMPLE)))
-        side = torch.cuda.Stream(device=dev)
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):                     # eager warm-up: kernel attributes, work-list uploads
-            _, n_s, _ = kde._density_body(self.x_in, preselected, fast)
-        torch.cuda.current_stream().wait_stream(side)
-        torch.cuda.synchronize()
-        if fast:
-            self.refs.append(eng._work_items(n_s))
-        gc.collect()
-        was_enabled = gc.isenabled()
-        gc.disable()                                      # no graph / pool destruction in the middle of the capture
-        try:
-            self.graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(self.graph, capture_error_mode="thread_local"):
-                self.packed, self.n_s, self.q = kde._density_body(self.x_in, preselected, fast)
-        finally:
-            if was_enabled:
-                gc.enable()
+
+        def body():
+            self.packed, self.n_s, self.q = kde._density_body(self.x_in, preselected, fast)
+
+        _, (self.graph,), self._keep_alive = E.capture_graphs([(body, True)], dev)
 
 
 class _PendingDensity:

@@ -628,9 +628,9 @@ class DSA(SA):
         self.class_matrix = self._class_matrix()
         self.badge_size = badge_size          # kept for API compatibility; tiles replace badges
         self.use_filter = os.environ.get("B200TIP_DSA_EXHAUSTIVE", "0") != "1"
-        self.use_graphs = os.environ.get("B200TIP_GRAPHS", "1") != "0"   # CUDA-graph replay of the search
+        self.use_graphs = E.GRAPHS            # CUDA-graph replay of the search
         self.capture_on_first_call = False
-        self._seen_shapes = set()
+        self._seen_shapes = E.BoundedCache(65)
         self._comm = comm
         self._engine = None
         self._engine_wide = None      # float64 twin for float64 test traces against float32 training traces
@@ -738,11 +738,7 @@ class DSA(SA):
         # pipeline scores most datasets exactly once (handler_surprise.py:84-99) and a capture costs ~3 eager
         # calls; its CUDA-graph plan is captured on the second sighting and replayed from then on.
         shape_key = (int(order.size), n_total, q_off.tobytes(), str(torch_dtype))
-        fused = self.use_graphs and (shape_key in self._seen_shapes or self.capture_on_first_call)
-        if self.use_graphs and not fused:
-            if len(self._seen_shapes) > 64:
-                self._seen_shapes.clear()
-            self._seen_shapes.add(shape_key)
+        fused = self.use_graphs and (self.capture_on_first_call or self._seen_shapes.touch(shape_key))
         if fused:
             # steady state: upload the permutation, replay, one D2H copy into pinned memory
             plan = E.dsa_plan(eng, int(order.size), q_off, x_all.dtype, self.use_filter,

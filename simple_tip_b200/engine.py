@@ -18,6 +18,7 @@ CPU (gloo, world_size 2).
 from __future__ import annotations
 
 import ctypes as C
+import gc
 import math
 import os
 import re
@@ -99,6 +100,78 @@ def host_array(x) -> np.ndarray:
 
 NP_DTYPE = {torch.float32: np.dtype(np.float32), torch.float64: np.dtype(np.float64),
             torch.float16: np.dtype(np.float16), torch.bfloat16: None}
+
+GRAPHS = os.environ.get("B200TIP_GRAPHS", "1") != "0"   # CUDA-graph replay of repeated batch shapes
+
+
+class BoundedCache(dict):
+    """A dict of at most `capacity` entries: a new key that would exceed it drops the oldest entry first."""
+
+    def __init__(self, capacity: int):
+        super().__init__()
+        self.capacity = capacity
+
+    def get_or_make(self, key, make):
+        if key not in self:
+            if len(self) >= self.capacity:
+                del self[next(iter(self))]
+            self[key] = make()
+        return self[key]
+
+    def touch(self, key) -> bool:
+        """True if `key` was seen before; records it either way (the seen-shape sets)."""
+        seen = key in self
+        self.get_or_make(key, lambda: None)
+        return seen
+
+
+_capture_keep: Optional[list] = None     # while capture_graphs captures: the tensors its graphs must keep alive
+
+
+def keep_for_capture(*tensors) -> None:
+    """Called by code that hands out a cached or engine-owned tensor.  While a CUDA graph is captured, the plan keeps
+    the tensor alive, since the graph bakes in its address and a cache may evict it later.  Otherwise a no-op."""
+    if _capture_keep is not None:
+        _capture_keep.extend(t for t in tensors if t is not None)
+
+
+def capture_graphs(segments, dev: torch.device) -> Tuple[list, list, list]:
+    """segments: [(fn, capturable)].  Every fn runs once eagerly on a side stream (fills caches, sets kernel
+    attributes, runs the collectives once); then each capturable fn is captured as a CUDA graph and every other fn
+    runs eagerly again, which keeps the ranks' collective sequences aligned.  Returns (steps: one callable per
+    segment, the graphs, the tensors keep_for_capture collected)."""
+    global _capture_keep
+    side = torch.cuda.Stream(device=dev)
+    side.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(side):
+        for fn, _ in segments:
+            fn()
+    torch.cuda.current_stream().wait_stream(side)
+    torch.cuda.synchronize()
+    steps, graphs, keep = [], [], []
+    # garbage from earlier plans (graphs, their private pools) must not be released in the middle of a capture:
+    # a cudaFree or a graph destroy there invalidates it
+    gc.collect()
+    was_enabled = gc.isenabled()
+    gc.disable()
+    try:
+        for fn, capturable in segments:
+            if not capturable:
+                fn()
+                steps.append(fn)
+                continue
+            g = torch.cuda.CUDAGraph()
+            _capture_keep = keep
+            with torch.cuda.graph(g, capture_error_mode="thread_local"):
+                fn()
+            _capture_keep = None
+            steps.append(g.replay)
+            graphs.append(g)
+    finally:
+        _capture_keep = None
+        if was_enabled:
+            gc.enable()
+    return steps, graphs, keep
 
 
 # ------------------------------------------------------------------------------------------
@@ -628,7 +701,7 @@ class NnEngine:
         self.num_classes = self.class_off.shape[0] - 1
         self.class_off_dev = torch.from_numpy(self.class_off.astype(np.int32)).to(self.dev)
         self.max_class_rows = int(np.diff(self.class_off).max()) if self.num_classes > 0 else 0
-        self._q_off_dev = {}
+        self._q_off_dev = BoundedCache(65)
         self.t_gid = t_gid.to(torch.int32).contiguous()
         self.cap = int(cap) if cap else (DEFAULT_CAP if self.d <= 256 else DEFAULT_CAP_LONG)
         self.pitch = int(self.lib.tip_pair_pitch(self.d, 1))
@@ -640,11 +713,10 @@ class NnEngine:
         self.row_tile, self.col_tile = qt.value, tt.value
         self.resident = int(self.lib.tip_nn_filter_kind(self.d)) == 1     # resident-query kernel (short traces)
         self.stats = torch.zeros(2, dtype=torch.int64, device=self.dev)
-        self._item_cache = {}
-        self._plans = {}
-        self._work = {}
-        self._inputs = {}
-        self._capture_refs = None     # while a plan is being captured: engine-owned tensors its graph reads
+        self._item_cache = BoundedCache(65)
+        self._plans = BoundedCache(8)
+        self._work = BoundedCache(16)
+        self._inputs = BoundedCache(8)
         self.sched_counter = torch.zeros(2, dtype=torch.int32, device=self.dev)
         self.last_cand_cnt_by_mode = {}
         # N_train-sharded engines: the whole (post-subsample) training set in ORIGINAL row order, replicated on
@@ -739,27 +811,17 @@ class NnEngine:
 
     def work_buffer(self, m: int, dtype: torch.dtype) -> torch.Tensor:
         """Scratch of tip_nn_rerank for m queries: zero-filled once, every call leaves it re-armed."""
-        key = (int(m), dtype)
-        w = self._work.get(key)
-        if w is None:
-            if len(self._work) >= 16:
-                self._work.clear()
+        def make():
             nbytes = int(self.lib.tip_nn_rerank_work_bytes(m, tip_dtype(dtype)))
-            w = torch.zeros(nbytes, dtype=torch.uint8, device=self.dev)
-            self._work[key] = w
-        return w
+            return torch.zeros(nbytes, dtype=torch.uint8, device=self.dev)
+
+        return self._work.get_or_make((int(m), dtype), make)
 
     def input_buffer(self, rows: int, dtype: torch.dtype) -> torch.Tensor:
         """Persistent HBM landing buffer for a batch of `rows` test traces (the H2D target of
         DSA.__call__ and the gather source of the captured search)."""
-        key = (int(rows), dtype)
-        b = self._inputs.get(key)
-        if b is None:
-            if len(self._inputs) >= 8:
-                self._inputs.pop(next(iter(self._inputs)))
-            b = torch.zeros((rows, self.d), dtype=dtype, device=self.dev)
-            self._inputs[key] = b
-        return b
+        return self._inputs.get_or_make((int(rows), dtype),
+                                        lambda: torch.zeros((rows, self.d), dtype=dtype, device=self.dev))
 
     def ranges(self, mode: int):
         off = self.class_off
@@ -792,15 +854,9 @@ class NnEngine:
         """Stage-1 winner positions of class-sorted inputs -> the stage-2 queries once per distinct winner
         (tip_dsa_distinct_winners): (rows, packed query state, slot_class, live_end, k, slot)."""
         m = pos.shape[0]
-        key = np.asarray(q_off, dtype=np.int64).tobytes()
-        q_off_dev = self._q_off_dev.get(key)
-        if q_off_dev is None:
-            if len(self._q_off_dev) > 64:
-                self._q_off_dev.clear()
-            q_off_dev = torch.from_numpy(np.asarray(q_off, dtype=np.int32)).to(self.dev)
-            self._q_off_dev[key] = q_off_dev
-        if self._capture_refs is not None:
-            self._capture_refs.extend(t for t in (q_off_dev, self.seed_b) if t is not None)
+        q_off_dev = self._q_off_dev.get_or_make(np.asarray(q_off, dtype=np.int64).tobytes(),
+                                                lambda: torch.from_numpy(np.asarray(q_off, dtype=np.int32)).to(self.dev))
+        keep_for_capture(q_off_dev, self.seed_b)
         rows = torch.empty((m, self.d), dtype=self.t.dtype, device=self.dev)
         state = self.query_state(m)
         slot_class, live_end, slot = (torch.empty(m, dtype=torch.int32, device=self.dev) for _ in range(3))
@@ -851,8 +907,8 @@ class NnEngine:
         if use_filter and self.n > 0:
             ranges = self.ranges(mode)
             key = (mode, np.asarray(q_off, dtype=np.int64).tobytes(), live_end is not None)
-            plan = self._item_cache.get(key)
-            if plan is None:       # host planning + upload once per (mode, class histogram)
+
+            def make():            # host planning + upload once per (mode, class histogram)
                 mixed = mode == _lib.RANGE_OTHER_CLASSES and self.other_class_mixed(q_off, m)
                 if live_end is not None:
                     assert self.resident and not mixed
@@ -875,12 +931,10 @@ class NnEngine:
                                            for c in range(self.num_classes))
                 flagged = bool(items.shape[0] and (items[:, 5] & 1).any())
                 n_static = items.shape[0] if n_static is None else n_static
-                plan = (torch.from_numpy(items).to(self.dev) if items.shape[0] else None, items.shape[0], flops, flagged,
+                return (torch.from_numpy(items).to(self.dev) if items.shape[0] else None, items.shape[0], flops, flagged,
                         n_static)
-                if len(self._item_cache) > 64:
-                    self._item_cache.clear()
-                self._item_cache[key] = plan
-            items_dev, n_items, flops, flagged, n_static = plan
+
+            items_dev, n_items, flops, flagged, n_static = self._item_cache.get_or_make(key, make)
             if n_items > 0:
                 if prepacked is not None:
                     q_pack, q_sq, q_err, row_min, cand_cnt = prepacked
@@ -906,17 +960,11 @@ class NnEngine:
                     name = "nn_filter_same_class" if mode == _lib.RANGE_SAME_CLASS else "nn_filter_other_classes"
                     PROFILE.append((name, flops, ev[0], ev[1]))
         work = self.work_buffer(m, q.dtype)
-        if self._capture_refs is not None:
-            # cached tensors whose addresses get baked into the graph: the plan keeps them alive even
-            # if the engine's caches evict them later
-            self._capture_refs.extend(t for t in (work, self.sched_counter, self.t_pack, self.t, self.t_gid,
-                                                  self.class_off_dev, self.center,
-                                                  items_dev if (use_filter and self.n > 0) else None) if t is not None)
         nq = [_p(t) for t in next_query] if next_query is not None else [None] * 5
         # stage 1 -> stage 2 hand-over: the winners' fit-time bounds seed the other-class search's running minima
         seed = self.seed_b if (next_query is not None and mode == _lib.RANGE_SAME_CLASS) else None
-        if self._capture_refs is not None and seed is not None:
-            self._capture_refs.append(seed)
+        keep_for_capture(work, self.sched_counter, self.t_pack, self.t, self.t_gid, self.class_off_dev, self.center,
+                         items_dev if (use_filter and self.n > 0) else None, seed)
         ex = _lib.RerankExtras()
         ex.q_idx = 0 if q_idx is None else q_idx.data_ptr()
         ex.next_seed_ub = 0 if seed is None else seed.data_ptr()
@@ -1038,34 +1086,6 @@ def dsa_distances(engine: NnEngine, x: torch.Tensor, q_class: torch.Tensor, q_of
     return dist_a, dist_b, gid
 
 
-class _Capture:
-    """Context for capturing engine work into a CUDA graph: garbage from earlier engines (old graphs,
-    their private pools) must not be released in the middle of the capture — a cudaFree / graph
-    destroy there invalidates it — and engine-owned tensors whose addresses get baked into the
-    graph are kept alive by the plan."""
-
-    def __init__(self, engine: "NnEngine", keep: list):
-        self.engine, self.keep = engine, keep
-
-    def __enter__(self):
-        import gc
-
-        gc.collect()
-        self.was_enabled = gc.isenabled()
-        gc.disable()
-        self.engine._capture_refs = []
-        return self
-
-    def __exit__(self, *exc):
-        import gc
-
-        self.keep.extend(self.engine._capture_refs)
-        self.engine._capture_refs = None
-        if self.was_enabled:
-            gc.enable()
-        return False
-
-
 class DsaPlan:
     """The whole scoring call for one (batch size, class histogram) captured as CUDA graph(s):
     gather into class-sorted order -> pack -> filter -> re-rank(+winner rows) -> pack -> filter ->
@@ -1110,7 +1130,6 @@ class DsaPlan:
         self.speculative = bool(use_filter and not sharded)
         self.overflow = engine.work_buffer(self.m, dtype)[:4].view(torch.int32)
         self.overflow_host = torch.zeros(1, dtype=torch.int32).pin_memory()
-        self._keep_alive = []
         S = self.state = {}
 
         def gather():
@@ -1189,28 +1208,8 @@ class DsaPlan:
 
             segments = [(seg_a, True), (exch_1, False), (seg_b, True), (exch_2, False), (seg_c, True)]
 
-        # eager warm-up on a side stream: fills caches, sets kernel attributes, runs the collectives once
-        side = torch.cuda.Stream(device=dev)
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):
-            for fn, _ in segments:
-                fn()
-        torch.cuda.current_stream().wait_stream(side)
-        torch.cuda.synchronize()
-        self.steps = []
-        for fn, capturable in segments:
-            if capturable:
-                g = torch.cuda.CUDAGraph()
-                with _Capture(engine, self._keep_alive):
-                    with torch.cuda.graph(g, capture_error_mode="thread_local"):
-                        fn()
-                self.steps.append(g.replay)
-            else:
-                fn()                      # keeps the ranks' collective sequences aligned during set-up
-                self.steps.append(fn)
-        self.graph = None
-        if len(segments) == 1:
-            self.graph = g
+        self.steps, graphs, self._keep_alive = capture_graphs(segments, dev)
+        self.graph = graphs[0] if len(segments) == 1 else None
         if self.speculative:
             self.overflow.zero_()     # whatever the warm-up ran on (a stale landing buffer) does not count
 
@@ -1243,13 +1242,7 @@ def dsa_plan(engine: "NnEngine", m: int, q_off: np.ndarray, dtype: torch.dtype, 
     n_total = int(m if n_total is None else n_total)
     key = (m, n_total, np.asarray(q_off, dtype=np.int64).tobytes(), dtype, use_filter, engine.cap, comm is not None,
            engine.table_b is not None)
-    plan = engine._plans.get(key)
-    if plan is None:
-        if len(engine._plans) >= 8:
-            engine._plans.pop(next(iter(engine._plans)))
-        plan = DsaPlan(engine, m, q_off, dtype, use_filter, comm, n_total=n_total)
-        engine._plans[key] = plan
-    return plan
+    return engine._plans.get_or_make(key, lambda: DsaPlan(engine, m, q_off, dtype, use_filter, comm, n_total=n_total))
 
 
 # ------------------------------------------------------------------------------------------
@@ -1300,23 +1293,20 @@ class KdeEngine:
         self.fast_ok = int(self.flags.item()) == 0 and self.comm is None
         if not self.fast_ok:
             self.t_pack_f16 = None
-        self._items = {}
+        self._items = BoundedCache(17)
 
     def _work_items(self, m: int):
         """Host planning + upload once per batch size."""
-        plan = self._items.get(m)
-        if plan is None:
+        def make():
             q_off = np.array([0, m], dtype=np.int64)
             ranges = [[(0, self.n)]]
             rt = int(self.lib.tip_kde_tile_rows())
             items, slots = build_items(q_off, ranges, span_tiles_for(count_tile_pairs(q_off, ranges, rt), self.sms), rt)
             items = span_major(items)
-            if len(self._items) > 16:
-                self._items.clear()
             # one partial per column part of a tile (tip_kde_slot_parts: 4 x 64 columns)
-            plan = (torch.from_numpy(items).to(self.dev), items.shape[0], slots * int(self.lib.tip_kde_slot_parts()))
-            self._items[m] = plan
-        return plan
+            return torch.from_numpy(items).to(self.dev), items.shape[0], slots * int(self.lib.tip_kde_slot_parts())
+
+        return self._items.get_or_make(m, make)
 
     def log_kernel_sum(self, q: torch.Tensor, fast: bool = False) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """q: [m, d] fp32 whitened, centred queries on the GPU.  Returns (mx, sm, qsq) with
@@ -1335,6 +1325,7 @@ class KdeEngine:
             _lib.check(lib.tip_pair_prep(_p(q), _lib.TIP_F32, m, self.d, None, _lib.ROLE_QUERY, 3, 1.0, 0.0, _p(q_pack),
                                          _p(q_sq), None, _stream()), "tip_pair_prep")
         items_dev, n_items, slots = self._work_items(m)
+        keep_for_capture(items_dev, self.t_pack, self.t_pack_f16, self.flags)
         part_max = torch.full((slots, m), float("-inf"), dtype=torch.float32, device=self.dev)
         part_sum = torch.zeros((slots, m), dtype=torch.float32, device=self.dev)
         if fast:
