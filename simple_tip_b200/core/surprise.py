@@ -688,61 +688,20 @@ class DSA(SA):
 
         from .. import engine as E
 
-        target_pred = _class_predictions(E.host_array(predictions))
-        dev_ats = E.device_matrix(activations)        # traces already in HBM: no host round trip
-        # NumPy promotes `from_ats[:, None] - to_ats` (surprise.py:638): float64 test traces against float32
-        # training traces are scored in float64 (the training traces widened exactly) -> a float64 twin of the
-        # engine, built on first use
-        wide = (dev_ats.dtype == torch.float64) if dev_ats is not None else \
-            (np.result_type(_flatten_layers(activations).dtype, self._compute_dtype) == np.float64)
-        compute = np.dtype(np.float64) if wide else self._compute_dtype
-        eng = self._engine
-        if compute != self._compute_dtype:
-            return self._call_promoted(activations, dev_ats, target_pred)
-        torch_dtype = torch.float64 if compute == np.float64 else torch.float32
-        if dev_ats is not None:
-            target_ats = dev_ats.to(torch_dtype)
-        else:
-            target_ats = _flatten_layers(activations)
-            if target_ats.dtype != compute:
-                target_ats = target_ats.astype(compute)
-        self._last_dtype = compute
-        dev = eng.dev
-        if target_ats.ndim != 2 or int(target_ats.shape[1]) != eng.d:
-            # the reference's `from_ats[:, None] - to_ats` raises the same kind of error (surprise.py:638)
-            raise ValueError(f"operands could not be broadcast together: test traces have shape "
-                             f"{tuple(target_ats.shape)}, training traces have {eng.d} features")
-        n_total = target_pred.shape[0]
-        sharded = self._comm is not None and self._comm.world > 1
-        # start the (asynchronous, if the caller's buffer is pinned) upload first; the host-side
-        # planning below overlaps with it
-        x_all = None
-        if n_total:
-            x_all = eng.input_buffer(n_total, torch_dtype)
-            x_all.copy_(target_ats if dev_ats is not None else torch.from_numpy(np.ascontiguousarray(target_ats)),
-                        non_blocking=True)
-        # class-grouped order; rows labelled >= num_classes are never scored by the reference
-        # (its result buffer is np.empty there, surprise.py:576-580) -> NaN here.
-        order, q_off = E.class_layout(target_pred, int(self.num_classes))
-        for c in range(int(self.num_classes)):
-            if q_off[c + 1] > q_off[c]:
-                if len(self.class_matrix[c]) == 0:
-                    raise ValueError("zero-size array to reduction operation minimum which has no identity")
-                if len(self.class_matrix[c]) == self.train_predictions.shape[0]:
-                    raise ValueError("zero-size array to reduction operation minimum which has no identity")
-        if order.size == 0:
-            self._last_raw = np.full((3, n_total), np.nan)
+        x_all, order, q_off, labels, promoted = self._prepare(activations, predictions)
+        n_total, eng = labels.shape[0], self._engine
+        if order.size == 0:       # no row to score
+            self._last_raw = np.full((4, n_total), np.nan)
             self._last_raw[2] = -1.0
-            return np.full(shape=n_total, fill_value=np.nan)
+            return self._last_raw[3].copy()
+        comm = self._comm if (self._comm is not None and self._comm.world > 1) else None
         # A batch shape (size, class histogram) seen for the first time is launched eagerly — the reference's
         # pipeline scores most datasets exactly once (handler_surprise.py:84-99) and a capture costs ~3 eager
         # calls; its CUDA-graph plan is captured on the second sighting and replayed from then on.
-        shape_key = (int(order.size), n_total, q_off.tobytes(), str(torch_dtype))
-        fused = self.use_graphs and (self.capture_on_first_call or self._seen_shapes.touch(shape_key))
-        if fused:
+        shape_key = (int(order.size), n_total, q_off.tobytes(), str(x_all.dtype))
+        if not promoted and self.use_graphs and (self.capture_on_first_call or self._seen_shapes.touch(shape_key)):
             # steady state: upload the permutation, replay, one D2H copy into pinned memory
-            plan = E.dsa_plan(eng, int(order.size), q_off, x_all.dtype, self.use_filter,
-                              self._comm if sharded else None, n_total=n_total)
+            plan = E.dsa_plan(eng, int(order.size), q_off, x_all.dtype, self.use_filter, comm, n_total=n_total)
             if plan.x_in.data_ptr() != x_all.data_ptr():
                 # the engine recycled its landing buffer since this plan was captured (many batch sizes)
                 plan.x_in.copy_(x_all)
@@ -753,26 +712,69 @@ class DSA(SA):
             plan.fetch_overflow()
             torch.cuda.current_stream().synchronize()
             if not plan.overflowed():
-                # the division already happened on the device in the trace dtype (surprise.py:595);
-                # last_dist_a / last_dist_b / last_winner_index read this buffer on demand
                 self._last_raw = plan.out_host.numpy()
                 return self._last_raw[3].copy()
             # some candidate list was empty or overflowed (heavy ties): the replayed graph carries no exhaustive-scan
-            # launches, so this call is repeated on the eager path below, which does
+            # launches, so this call is repeated eagerly below, which does
             plan.clear_overflow()
-        idx = torch.from_numpy(order).to(dev, non_blocking=True)
-        x = x_all.index_select(0, idx)
-        q_class = torch.from_numpy(target_pred[order].astype(np.int32)).to(dev, non_blocking=True)
-        dist_a, dist_b, gid = E.dsa_distances(eng, x, q_class, q_off, self._comm if sharded else None, self.use_filter)
-        packed = torch.stack([dist_a.to(torch.float64), dist_b.to(torch.float64), gid.to(torch.float64)])
-        # back to the caller's order on the device, then a single D2H transfer
-        # (float32/float64 -> float64 and int -> float64 are exact)
-        full = torch.full((3, n_total), float("nan"), dtype=torch.float64, device=dev)
-        full[2].fill_(-1.0)
-        full.index_copy_(1, idx, packed)
-        return self._finish(full.cpu().numpy())
+        idx = torch.from_numpy(order.astype(np.int32)).to(eng.dev, non_blocking=True)
+        q_class = torch.from_numpy(labels[order].astype(np.int32)).to(eng.dev, non_blocking=True)
+        out = torch.empty((4, n_total), dtype=torch.float64, device=eng.dev)
+        if promoted:
+            self._call_promoted(x_all, idx, q_class, q_off, out)
+        else:
+            E.dsa_scores(eng, x_all, idx, q_class, q_off, out, comm, self.use_filter)
+        self._last_raw = out.cpu().numpy()
+        return self._last_raw[3].copy()
 
-    def _call_promoted(self, activations, dev_ats, target_pred) -> np.ndarray:
+    def _prepare(self, activations, predictions):
+        """The checks and the upload every call shares.  Returns the test traces in the engine's landing buffer (in the
+        scoring dtype), the class-grouped order and offsets of the rows to score, the labels, and whether the call
+        is promoted (float64 test traces against float32 training traces)."""
+        import torch
+
+        from .. import engine as E
+
+        labels = _class_predictions(E.host_array(predictions))
+        dev_ats = E.device_matrix(activations)        # traces already in HBM: no host round trip
+        host_ats = _flatten_layers(activations) if dev_ats is None else None
+        # NumPy promotes `from_ats[:, None] - to_ats` (surprise.py:638): float64 test traces against float32
+        # training traces are scored in float64 (the training traces widened exactly)
+        wide = (dev_ats.dtype == torch.float64) if dev_ats is not None else \
+            (np.result_type(host_ats.dtype, self._compute_dtype) == np.float64)
+        compute = np.dtype(np.float64) if wide else self._compute_dtype
+        promoted = compute != self._compute_dtype
+        if promoted and self._comm is not None and self._comm.world > 1:
+            raise TypeError("N_train-sharded DSA scores in the dtype of the training traces "
+                            f"({self._compute_dtype}); got float64 test traces")
+        torch_dtype = torch.float64 if compute == np.float64 else torch.float32
+        if dev_ats is not None:
+            target_ats = dev_ats.to(torch_dtype)
+        else:
+            target_ats = host_ats if host_ats.dtype == compute else host_ats.astype(compute)
+        eng = self._engine
+        if target_ats.ndim != 2 or int(target_ats.shape[1]) != eng.d:
+            # the reference's `from_ats[:, None] - to_ats` raises the same kind of error (surprise.py:638)
+            raise ValueError(f"operands could not be broadcast together: test traces have shape "
+                             f"{tuple(target_ats.shape)}, training traces have {eng.d} features")
+        n_total = labels.shape[0]
+        # start the (asynchronous, if the caller's buffer is pinned) upload first; the host-side
+        # planning below overlaps with it
+        x_all = None
+        if n_total:
+            x_all = eng.input_buffer(n_total, torch_dtype)
+            x_all.copy_(target_ats if dev_ats is not None else torch.from_numpy(np.ascontiguousarray(target_ats)),
+                        non_blocking=True)
+        # class-grouped order; rows labelled >= num_classes are never scored by the reference
+        # (its result buffer is np.empty there, surprise.py:576-580) -> NaN here.
+        order, q_off = E.class_layout(labels, int(self.num_classes))
+        for c in range(int(self.num_classes)):
+            if q_off[c + 1] > q_off[c] and len(self.class_matrix[c]) in (0, self.train_predictions.shape[0]):
+                raise ValueError("zero-size array to reduction operation minimum which has no identity")
+        self._last_dtype = compute
+        return x_all, order, q_off, labels, promoted
+
+    def _call_promoted(self, x_all, idx, q_class, q_off, out):
         """float64 test traces against float32 training traces, exactly as NumPy promotes them in the reference:
         stage 1 (`from_ats[:, None] - to_ats`, surprise.py:638) runs in float64 on the exactly widened training traces
         (a float64 twin of the engine, built on first use); stage 2's operands are both float32 TRAINING rows, so it
@@ -782,48 +784,17 @@ class DSA(SA):
         from .. import _lib
         from .. import engine as E
 
-        if self._comm is not None and self._comm.world > 1:
-            raise TypeError("N_train-sharded DSA scores in the dtype of the training traces "
-                            f"({self._compute_dtype}); got float64 test traces")
         if self._engine_wide is None:
             train = self.train_activations
             train = train.to(torch.float64) if isinstance(train, torch.Tensor) else np.asarray(train, dtype=np.float64)
             self._engine_wide = E.NnEngine.from_host(train, self.train_predictions, int(self.num_classes),
                                                      np.arange(train.shape[0]), seeds=False)
         eng, wide = self._engine, self._engine_wide
-        dev = eng.dev
-        x_all = dev_ats.to(torch.float64) if dev_ats is not None else \
-            E.to_device(_flatten_layers(activations).astype(np.float64), dev)
-        if x_all.ndim != 2 or int(x_all.shape[1]) != eng.d:
-            raise ValueError(f"operands could not be broadcast together: test traces have shape {tuple(x_all.shape)}, "
-                             f"training traces have {eng.d} features")
-        n_total = target_pred.shape[0]
-        order, q_off = E.class_layout(target_pred, int(self.num_classes))
-        for c in range(int(self.num_classes)):
-            if q_off[c + 1] > q_off[c] and len(self.class_matrix[c]) in (0, self.train_predictions.shape[0]):
-                raise ValueError("zero-size array to reduction operation minimum which has no identity")
-        self._last_dtype = np.dtype(np.float64)
-        full = np.full((3, n_total), np.nan)
-        full[2] = -1.0
-        if order.size:
-            idx = torch.from_numpy(order).to(dev)
-            x = x_all.index_select(0, idx)
-            q_class = torch.from_numpy(target_pred[order].astype(np.int32)).to(dev)
-            dist_a, pos, gid, _ = wide.search(x, q_class, q_off, _lib.RANGE_SAME_CLASS, self.use_filter)
-            winners = eng.gather(pos)                      # float32 training rows (same class-sorted positions)
-            dist_b = eng.search(winners, q_class, q_off, _lib.RANGE_OTHER_CLASSES, self.use_filter)[0]
-            packed = torch.stack([dist_a, dist_b.to(torch.float64), gid.to(torch.float64)]).cpu().numpy()
-            full[:, order] = packed
-        return self._finish(full)
-
-    def _finish(self, res: np.ndarray) -> np.ndarray:
-        """res[3, n]: dist_a, dist_b, winner index as float64 (exact widenings) in the caller's order."""
-        self._last_raw = res
-        a = res[0].astype(self._last_dtype or self._compute_dtype)
-        b = res[1].astype(self._last_dtype or self._compute_dtype)
-        with np.errstate(divide="ignore", invalid="ignore"):
-            # the reference divides in the input dtype and widens on store (surprise.py:595,611)
-            return (a / b).astype(np.float64)
+        dist_a, pos, gid, _ = wide.search(x_all, q_class, q_off, _lib.RANGE_SAME_CLASS, self.use_filter, q_idx=idx)
+        winners = eng.gather(pos)                      # float32 training rows (same class-sorted positions)
+        dist_b = eng.search(winners, q_class, q_off, _lib.RANGE_OTHER_CLASSES, self.use_filter)[0]
+        E.reset_unscored(out, idx.shape[0])
+        E.pack_out(dist_a, dist_b.to(torch.float64), gid, idx, out)
 
     # Results of the most recent call (exact widenings of the device values; valid until the next call)
     @property

@@ -988,11 +988,16 @@ class NnEngine:
         return out_dist, out_pos, out_gid, out_rows
 
     def gather(self, pos: torch.Tensor) -> torch.Tensor:
-        out = torch.empty((pos.shape[0], self.d), dtype=self.t.dtype, device=self.dev)
-        if pos.shape[0]:
-            _lib.check(self.lib.tip_gather_rows(_p(self.t), self.d * self.t.element_size(), _p(pos), pos.shape[0],
-                                                _p(out), _stream()), "tip_gather_rows")
-        return out
+        return gather_rows(self.t, pos)
+
+
+def gather_rows(src: torch.Tensor, pos: torch.Tensor) -> torch.Tensor:
+    """src[pos] for int32 row positions `pos` (tip_gather_rows)."""
+    out = torch.empty((pos.shape[0], src.shape[1]), dtype=src.dtype, device=src.device)
+    if pos.shape[0]:
+        _lib.check(_lib.load().tip_gather_rows(_p(src), src.shape[1] * src.element_size(), _p(pos), pos.shape[0],
+                                               _p(out), _stream()), "tip_gather_rows")
+    return out
 
 
 def winner_queries(engine: "NnEngine", p2p: Optional[P2PExchange], gdist: Optional[torch.Tensor],
@@ -1031,8 +1036,7 @@ def dsa_distances(engine: NnEngine, x: torch.Tensor, q_class: torch.Tensor, q_of
         dist_b = torch.where(found, engine.table_b.index_select(0, pos.clamp_min(0).to(torch.int64)),
                              torch.full_like(dist_a, float("nan")))
         if scatter is not None:
-            _lib.check(engine.lib.tip_dsa_pack_out(_p(dist_a), _p(dist_b), tip_dtype(dist_a.dtype), _p(gid), _p(scatter[0]),
-                                                   m, int(scatter[1]), _p(scatter[2]), _stream()), "tip_dsa_pack_out")
+            pack_out(dist_a, dist_b, gid, scatter[0], scatter[2])
         return dist_a, dist_b, gid
     if not sharded:
         fuse = use_filter and engine.has_items(q_off, _lib.RANGE_OTHER_CLASSES)
@@ -1086,17 +1090,47 @@ def dsa_distances(engine: NnEngine, x: torch.Tensor, q_class: torch.Tensor, q_of
     return dist_a, dist_b, gid
 
 
+def pack_out(dist_a: torch.Tensor, dist_b: torch.Tensor, gid: torch.Tensor, idx: Optional[torch.Tensor],
+             out: torch.Tensor) -> None:
+    """out[:, idx[r]] = (dist_a, dist_b, winner index, dist_a / dist_b) of class-sorted query r, as float64; the division
+    runs in the dtype of dist_a and dist_b (tip_dsa_pack_out)."""
+    _lib.check(_lib.load().tip_dsa_pack_out(_p(dist_a), _p(dist_b), tip_dtype(dist_a.dtype), _p(gid), _p(idx),
+                                            gid.shape[0], out.shape[1], _p(out), _stream()), "tip_dsa_pack_out")
+
+
+def reset_unscored(out: torch.Tensor, m: int) -> None:
+    """A call that scores m < n_total rows leaves the others NaN / -1; which rows those are can change between calls."""
+    if out.shape[1] != m:
+        out.fill_(float("nan"))
+        out[2].fill_(-1.0)
+
+
+def dsa_scores(engine: NnEngine, x_in: torch.Tensor, idx: torch.Tensor, q_class: torch.Tensor, q_off: np.ndarray,
+               out: torch.Tensor, comm: Optional[TrainShardComm] = None, use_filter: bool = True,
+               speculative: bool = False) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """One DSA scoring call on the device, the sequence DsaPlan captures.  x_in: [n_total, d] test traces in the
+    caller's row order; idx: int32 [m], the caller's row of every class-sorted query (classes by q_off, q_class[m]);
+    out: float64 [4, n_total] <- dist_a, dist_b, winner index, dist_a / dist_b in the caller's order, NaN / -1 in the
+    rows outside idx.  Returns dist_a, dist_b and the winner index in class-sorted order.  speculative: see
+    NnEngine.search (single shard only)."""
+    reset_unscored(out, idx.shape[0])
+    if comm is None or comm.world <= 1:
+        return dsa_distances(engine, x_in, q_class, q_off, None, use_filter, q_idx=idx,
+                             scatter=(idx, out.shape[1], out), speculative=speculative)
+    dist_a, dist_b, gid = dsa_distances(engine, gather_rows(x_in, idx), q_class, q_off, comm, use_filter)
+    pack_out(dist_a, dist_b, gid, idx, out)
+    return dist_a, dist_b, gid
+
+
 class DsaPlan:
-    """The whole scoring call for one (batch size, class histogram) captured as CUDA graph(s):
-    gather into class-sorted order -> pack -> filter -> re-rank(+winner rows) -> pack -> filter ->
-    re-rank -> scatter of (dist_a, dist_b, winner index) back to the caller's row order.
+    """The whole scoring call for one (batch size, class histogram), `dsa_scores`, captured as CUDA graph(s).
     Inputs: `x_in` [n_total, d] (the engine's landing buffer for host uploads) and `idx` [m]
     (original row of every class-sorted query).  Output: `out` [4, n_total] float64 in the
     caller's order — dist_a, dist_b, winner index, dist_a / dist_b (divided in the trace dtype) —
     where rows the reference never scores keep NaN / -1.
 
     N_train sharded (comm.world > 1): with the peer-memory exchange the two exchange steps are
-    kernels of ours and the call is still ONE graph; with the torch.distributed fallback the call is
+    kernels of ours and the call is still ONE graph; with the torch.distributed fallback the same steps run as
     three graph segments with one eager MIN all-reduce between consecutive segments (two for float64
     traces in the first exchange)."""
 
@@ -1106,19 +1140,16 @@ class DsaPlan:
         self.engine = engine
         self.q_off = np.asarray(q_off, dtype=np.int64).copy()
         dev = engine.dev
-        lib = engine.lib
         self.m = int(m)
         self.n_total = int(m if n_total is None else n_total)
         self.x_in = engine.input_buffer(self.n_total, dtype)
         self.idx = torch.arange(self.m, dtype=torch.int32, device=dev)
-        self.x = torch.zeros((m, engine.d), dtype=dtype, device=dev)
         self.out = torch.full((4, self.n_total), float("nan"), dtype=torch.float64, device=dev)
         self.out[2].fill_(-1.0)
         self.out_host = torch.empty((4, self.n_total), dtype=torch.float64).pin_memory()
         self.idx_host = torch.empty(self.m, dtype=torch.int32).pin_memory()
         q_class = np.repeat(np.arange(engine.num_classes, dtype=np.int32), np.diff(self.q_off))
         self.q_class = torch.from_numpy(q_class).to(dev)
-        row_bytes = engine.d * self.x.element_size()
         self.comm = comm if (comm is not None and comm.world > 1) else None
         sharded = self.comm is not None
         if sharded and engine.t_full is None:
@@ -1130,40 +1161,16 @@ class DsaPlan:
         self.speculative = bool(use_filter and not sharded)
         self.overflow = engine.work_buffer(self.m, dtype)[:4].view(torch.int32)
         self.overflow_host = torch.zeros(1, dtype=torch.int32).pin_memory()
-        S = self.state = {}
-
-        def gather():
-            _lib.check(lib.tip_gather_rows(_p(self.x_in), row_bytes, _p(self.idx), self.m, _p(self.x), _stream()),
-                       "tip_gather_rows")
-
-        def scatter(a, b, gid):
-            if self.n_total != self.m:         # which rows are unscored can change between calls
-                self.out.fill_(float("nan"))
-                self.out[2].fill_(-1.0)
-            _lib.check(lib.tip_dsa_pack_out(_p(a), _p(b), tip_dtype(a.dtype), _p(gid), _p(self.idx), self.m,
-                                            self.n_total, _p(self.out), _stream()), "tip_dsa_pack_out")
-            self.dist_a, self.dist_b, self.gid = a, b, gid
-
-        if not sharded:
+        if not sharded or self.p2p is not None:
             def whole():
-                # gather fused into the pack / re-rank (q_idx), result scatter fused into the last re-rank
-                if self.n_total != self.m:         # which rows are unscored can change between calls
-                    self.out.fill_(float("nan"))
-                    self.out[2].fill_(-1.0)
-                self.dist_a, self.dist_b, self.gid = dsa_distances(engine, self.x_in, self.q_class, self.q_off, None, use_filter,
-                                                                   q_idx=self.idx, scatter=(self.idx, self.n_total, self.out),
-                                                                   speculative=self.speculative)
-
-            segments = [(whole, True)]
-        elif self.p2p is not None:
-            def whole():
-                gather()
-                scatter(*dsa_distances(engine, self.x, self.q_class, self.q_off, self.comm, use_filter))
+                dsa_scores(engine, self.x_in, self.idx, self.q_class, self.q_off, self.out, self.comm, use_filter,
+                           self.speculative)
 
             segments = [(whole, True)]
         else:
             # torch.distributed fallback: static exchange buffers written by one graph segment,
             # all-reduced in place (eager), read by the next segment
+            S = self.state = {}
             f32 = dtype == torch.float32
             # distances travel as dist_keys (integers, "no row" above +inf), so a real +inf survives the exchange
             S["keys"] = torch.zeros(self.m, dtype=torch.int64, device=dev)
@@ -1172,8 +1179,8 @@ class DsaPlan:
             S["bmin"] = torch.zeros(self.m, dtype=torch.int32 if f32 else torch.int64, device=dev)
 
             def seg_a():
-                gather()
-                la, _, lg, _ = engine.search(self.x, self.q_class, self.q_off, _lib.RANGE_SAME_CLASS, use_filter)
+                x = gather_rows(self.x_in, self.idx)
+                la, _, lg, _ = engine.search(x, self.q_class, self.q_off, _lib.RANGE_SAME_CLASS, use_filter)
                 S["lg"] = lg
                 if f32:
                     S["keys"].copy_(pack_winner_keys(la, lg))
@@ -1204,7 +1211,8 @@ class DsaPlan:
                 self.comm.min_(S["bmin"])
 
             def seg_c():
-                scatter(S["a"], keys_dist(S["bmin"]), S["gid"])
+                reset_unscored(self.out, self.m)
+                pack_out(S["a"], keys_dist(S["bmin"]), S["gid"], self.idx, self.out)
 
             segments = [(seg_a, True), (exch_1, False), (seg_b, True), (exch_2, False), (seg_c, True)]
 
